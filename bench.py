@@ -1,14 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- fp64 block-matmul GFLOP/s at N=16384 (BASELINE.json metric), 1..8 B200.
+"""bench.py -- fp64 block-matmul GFLOP/s at N=16384 (BASELINE.json metric), 1..8 H100.
 
   python bench.py --gpus N --steps K --warmup W            our arm  (CUDA, through the C ABI)
   python bench.py --impl reference --gpus N ...            reference arm: the reference algorithm
-                                                           restated on the box's host cores (oracle/)
+                                                           restated on the host cores (oracle/)
 
 A "step" is one full C = A * B over the whole block matrix.  `value` is measured with the inputs
 resident in HBM; `e2e` is the same multiply through the public Dataset API with HOST buffers
 (host->device copies of every A and B block and device->host copies of every C block inside the
 timed region).  Prints ONE JSON line on rank 0.
+
+  --dump-outputs DIR   after the timed steps, writes a fixed seeded sample of the blocks of C the last timed step computed
+                       (DIR/C_blocks.npy, float64 [k, blk * blk], each row one block's column-major payload; DIR/C_block_ids.npy, [k, 2] block
+                       ids).  One GPU and the metric workload only.
+                       The operands come from fixed seeds, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -28,55 +33,13 @@ METRIC = "fp64 block-matmul GFLOP/s at N=16384"
 UNIT = "GFLOP/s"
 
 
+# Roofline denominators are NVIDIA's data-sheet figures for the H100 SXM at its 700 W limit -- ceilings, not measured rates.
 def fp64_peak_tflops():
-    """Roofline denominator for the fp64 tensor pipe: MEASURED_PEAKS.json has no fp64 entry, so the
-    measured DMMA peak of tools/fp64_peak.cu (profiles/fp64_peaks_r01.jsonl) is used."""
-    path = os.path.join(ROOT, "profiles", "fp64_peaks_r01.jsonl")
-    best, src = None, None
-    try:
-        for line in open(path):
-            d = json.loads(line)
-            if d.get("bench") == "dmma_sustained":
-                best, src = d["tflops"], "profiles/fp64_peaks_r01.jsonl dmma_sustained (measured on this pool's B200; MEASURED_PEAKS.json has no fp64 entry)"
-    except OSError:
-        pass
-    if best is None:
-        best, src = 37.2, "nominal 148 SM x 64 FMA/clk x 2 x 1.965 GHz (fallback: no measured file)"
-    return best, src
-
-
-def dram_traffic_per_launch(n: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the GEMM kernel at this N from the committed ncu capture
-    (profiles/gemm_traffic_r01.json), or None when no capture exists for this size."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "gemm_traffic_r01.json")))
-        e = d.get(str(n))
-        return None if e is None else {"bytes": e["dram_read_bytes"] + e["dram_write_bytes"], "algorithmic_bytes": 3 * n * n * 8,
-                                       "unit": "bytes per launch", "source": e.get("source", "ncu")}
-    except (OSError, ValueError, KeyError):
-        return None
-
-
-def tc_traffic_per_launch(n: int, moduli: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one ozaki2_gemm_2sm_kernel launch at this N and moduli count, from the
-    committed `ncu --set full` capture (profiles/gemm_traffic_r02.json), or None when no capture exists for this configuration.
-    Algorithmic bytes of the launch: the int8 residues of both operands read once (2 x T x N^2) + the residue planes written (T x N^2)."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "gemm_traffic_r02.json")))
-        e = d.get(f"{n}x{moduli}")
-        if e is None:
-            return None
-        scale = e.get("total_tiles", 1) / e.get("captured_tiles", 1)   # the capture holds one piece of the multiply's tile list
-        return {"bytes": (e["dram_read_bytes"] + e["dram_write_bytes"]) * scale, "algorithmic_bytes": 3 * moduli * n * n,
-                "captured_launch_bytes": e["dram_read_bytes"] + e["dram_write_bytes"], "captured_tiles": e.get("captured_tiles"),
-                "total_tiles": e.get("total_tiles"), "l2_hit_rate_pct": e.get("l2_hit_rate_pct"),
-                "unit": "bytes per step (all pieces of the multiply's tile list)", "source": e.get("source", "ncu")}
-    except (OSError, ValueError, KeyError, TypeError, ZeroDivisionError):
-        return None
+    return 67.0, "NVIDIA H100 SXM data sheet: 67 TFLOP/s FP64 tensor core, dense, 700 W (not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index: int):
         self.index, self.proc, self.lines, self.mark_at = index, None, [], 0
@@ -140,17 +103,15 @@ class ClockSampler:
 # reference arm / cpu_baseline: the reference ALGORITHM restated on host cores (oracle/)
 #
 # Both legs run in a SUBPROCESS (`bench.py --_cpu-worker ...`) whose environment pins every BLAS / OpenMP pool to one
-# thread BEFORE numpy loads, and whose parallelism is one forked worker PROCESS per host core.  (Round 1 ran 128 Python
-# threads into the numpy-bundled OpenBLAS, which is built for 64: "precompiled NUM_THREADS exceeded" -> heap corruption
-# -> rc 134 / 139 on the 128-thread GPU hosts, and a 4.5x swing of the reported baseline.)  The GPU process itself never
-# runs the CPU legs.
+# thread BEFORE numpy loads, and whose parallelism is one forked worker PROCESS per host core (more Python threads than the
+# numpy-bundled OpenBLAS is built for corrupt its heap).  The GPU process itself never runs the CPU legs.
 # ------------------------------------------------------------------------------------------------
 _W = {}
 
 
 def host_cores() -> int:
-    """Cores this process may actually use: the affinity mask, capped by the cgroup CPU quota (a 1-GPU lease of the 128-thread
-    GPU host gets a fraction of its CPUs: round 1 read 353 GFLOP/s there and 1600 on the 8-GPU lease of the same host class)."""
+    """Cores this process may actually use: the affinity mask, capped by the cgroup CPU quota (a container on a large host may
+    be granted a fraction of its CPUs)."""
     try:
         n = max(1, len(os.sched_getaffinity(0)))
     except AttributeError:
@@ -309,41 +270,36 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------------
-def tc_peaks():
-    """Measured tcgen05 peaks of tools/tc_peak.cu (profiles/tc_peaks_r02.jsonl): {bench: value}."""
-    out = {}
-    try:
-        for line in open(os.path.join(ROOT, "profiles", "tc_peaks_r02.jsonl")):
-            if line.startswith("{"):
-                d = json.loads(line)
-                out[d["bench"]] = d["value"]
-    except (OSError, ValueError, KeyError):
-        pass
-    return out
-
-
 def int8_peak_tops():
-    pk = tc_peaks()
-    if "tcgen05_i8_sustained" in pk:
-        return pk["tcgen05_i8_sustained"], ("profiles/tc_peaks_r02.jsonl tcgen05_i8_sustained (tools/tc_peak.cu: back-to-back 128x256x32 kind::i8 MMAs "
-                                            "on shared-memory operands, all SMs, ~3 s; MEASURED_PEAKS.json has no int8 entry)")
-    try:
-        bf16 = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"]
-        return 2.0 * bf16, "2 x MEASURED_PEAKS.json bf16_tflops_sustained (int8 dense = 2 x bf16 dense on this part; no int8 microbenchmark file)"
-    except (OSError, ValueError, KeyError):
-        return 2.0 * 1400.0, "2 x the profiling guide's sustained bf16 fallback (1.4 PFLOP/s)"
+    return 1979.0, "NVIDIA H100 SXM data sheet: 1979 TOPS INT8 tensor core, dense, 700 W (not measured)"
 
 
-def time_multiply(torch, stream, A, B, n, blk, steps):
+def time_multiply(torch, stream, A, B, n, blk, steps, keep_last=False):
+    """Mean milliseconds of `steps` multiplies; with keep_last also the product of the last timed step."""
     evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+    C = None
     for e0, e1 in evs:
+        del C
         e0.record(stream)
         C = A.matrixMultiply(n, n, B, n, n, blk)
         e1.record(stream)
-        del C
     torch.cuda.synchronize()
     ms = [e0.elapsed_time(e1) for e0, e1 in evs]
-    return sum(ms) / len(ms)
+    return sum(ms) / len(ms), (C if keep_last else None)
+
+
+DUMP_BYTES = 60 << 20   # --dump-outputs writes at most this much of C
+
+
+def dump_outputs(np, C, nb, blk, out_dir):
+    """A fixed seeded sample of whole blocks of C (all of them when they fit), payloads as stored (column-major)."""
+    ids = [(i, j) for i in range(nb) for j in range(nb)]
+    k = max(1, min(len(ids), DUMP_BYTES // (blk * blk * 8)))
+    pick = sorted(np.random.default_rng(0).choice(len(ids), size=k, replace=False).tolist())
+    blocks = np.stack([np.asarray(C.get_block(*ids[t]).values, dtype=np.float64).reshape(-1) for t in pick])
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "C_blocks.npy"), blocks)
+    np.save(os.path.join(out_dir, "C_block_ids.npy"), np.array([ids[t] for t in pick], dtype=np.float64))
 
 
 def run_ours(args):
@@ -355,13 +311,15 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 engine has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device; the engine has no CPU fallback")
     torch.cuda.set_device(local_rank)
     n, blk = args.n, args.blk
     nb = n // blk
     flops = 2.0 * n ** 3
 
     if world > 1:
+        if args.dump_outputs:
+            raise SystemExit("bench.py: --dump-outputs is supported on one GPU only")
         from matrel_b200 import distributed as dist_mm
         line = dist_mm.bench_main(args, METRIC, UNIT, fp64_peak_tflops, ClockSampler, cpu_reference_sample, int8_peak_tops)
         if line is not None:   # rank 0
@@ -390,10 +348,13 @@ def run_ours(args):
         torch.cuda.synchronize()
         sampler.mark()
         t_wall0 = time.perf_counter()
-        ms_per_step = time_multiply(torch, stream, A, B, n, blk, args.steps)
+        ms_per_step, C_last = time_multiply(torch, stream, A, B, n, blk, args.steps, keep_last=bool(args.dump_outputs))
         t_wall = time.perf_counter() - t_wall0
         clocks = sampler.stop()
         st = s.stats()
+        if args.dump_outputs:   # after the clocks and counters are read: the JSON line does not depend on the flag
+            dump_outputs(np, C_last, nb, blk, args.dump_outputs)
+        del C_last
         launches_per_step = st["kernel_launches"] / args.steps
         on_tc = st["tc_gemm_launches"] > 0
 
@@ -412,28 +373,27 @@ def run_ours(args):
             kern_ms = st2["tc_gemm_ms_total"] / reps
             ipeak, ipeak_src = int8_peak_tops()
             ach = st2["tc_int8_ops"] / (kern_ms * 1e-3) / 1e12
-            tct = tc_traffic_per_launch(n, moduli_used)
             # the engine's plane-capacity rule (csrc/abi_multiply.cpp: plane_cap_tiles, rounded up to an even tile count)
             plane_cap = max(64, (2 << 30) // (max(1, moduli_used) * 128 * 256))
             plane_cap += plane_cap & 1
             tiles_total = (-(-n // 128)) * (-(-n // 256))
             pieces = -(-tiles_total // plane_cap)
             roofline = {"bound": "tensor", "achieved": ach, "peak": ipeak, "unit": "TFLOP/s", "frac": ach / ipeak,
-                        "traffic": (tct or {}).get("bytes"), "traffic_detail": tct,
-                        "op": "int8 multiply-add x 2 (TOPS) on tcgen05.mma kind::i8, s32 accumulators in TMEM",
-                        "kernel": "ozaki2_gemm_2sm_kernel (persistent CTA pairs, TMA -> 6-stage smem ring -> UTCIMMA cta_group::2 256x256x32 -> TMEM -> residue epilogue)",
+                        "traffic": None,
+                        "op": "int8 multiply-add x 2 (TOPS) on wgmma s8, s32 accumulators in registers",
+                        "kernel": "ozaki2_gemm_2sm_kernel (persistent CTA pairs, TMA with B' multicast -> 4-stage smem ring -> wgmma m64n256k32 s8 -> residue epilogue)",
                         "kernel_ms": kern_ms, "launches_per_step": 1.0,
                         "algorithmic": f"{st2['tc_moduli']} moduli x 2*N^3 = {st2['tc_int8_ops']:.4g} int8 ops per step (all moduli x all tiles; the 2 GiB residue-plane "
                                        f"buffer holds {plane_cap} of the {tiles_total} 128x256 tiles at {moduli_used} moduli, so the step's GEMM is {pieces} back-to-back "
                                        "launch(es) of this kernel and kernel_ms is their sum)",
                         "peak_source": ipeak_src,
                         "fp64_equivalent": {"achieved": flops / (ms_per_step * 1e-3) / 1e12, "dmma_peak": dpeak, "x_dmma_roof": flops / (ms_per_step * 1e-3) / 1e12 / dpeak,
-                                            "note": "whole multiply (absmax + residues + int8 GEMM + CRT) as fp64 flop/s against the measured native-fp64 (DMMA) roof"}}
+                                            "note": "whole multiply (absmax + residues + int8 GEMM + CRT) as fp64 flop/s against the native-fp64 (DMMA) data-sheet roof"}}
         else:
             kern_ms = st2["gemm_ms_total"] / max(1, st2["gemm_launches"])
             ach = flops / (kern_ms * 1e-3) / 1e12
             roofline = {"bound": "tensor", "achieved": ach, "peak": dpeak, "unit": "TFLOP/s", "frac": ach / dpeak,
-                        "traffic": (dram_traffic_per_launch(n) or {}).get("bytes"), "traffic_detail": dram_traffic_per_launch(n),
+                        "traffic": None,
                         "kernel": "gemm_f64_dmma_kernel<128,128,2,4,5>", "kernel_ms": kern_ms, "launches_per_step": 1.0,
                         "algorithmic": f"2*N^3 = {flops:.4g} flop per launch (whole block multiply, K reduction fused)", "peak_source": dpeak_src}
 
@@ -461,7 +421,7 @@ def run_ours(args):
                     del C
                 s.sync()
                 d_steps = max(3, min(args.steps, 5))
-                d_ms = time_multiply(torch, stream, A, B, n, blk, d_steps)
+                d_ms, _ = time_multiply(torch, stream, A, B, n, blk, d_steps)
                 Cd = A.matrixMultiply(n, n, B, n, n, blk)
                 s.set_option("gemm_algo", args.algo)
                 Ct = A.matrixMultiply(n, n, B, n, n, blk)
@@ -470,12 +430,11 @@ def run_ours(args):
                     a_, b_ = Cd.get_block(*key).values, Ct.get_block(*key).values
                     worst = max(worst, float(np.max(np.abs(a_ - b_)) / np.max(np.abs(a_))))
                 del Cd, Ct
-                tr = dram_traffic_per_launch(n)
                 dmma = {"algo": "gemm_algo 1: gemm_f64_dmma_kernel (TMA -> 5-stage ring -> mma.sync m8n8k4 f64)", "value": flops / (d_ms * 1e-3) / 1e9,
                         "unit": UNIT, "ms_per_step": d_ms, "steps": d_steps,
                         "roofline": {"bound": "tensor", "achieved": flops / (d_ms * 1e-3) / 1e12, "peak": dpeak, "unit": "TFLOP/s",
-                                     "frac": flops / (d_ms * 1e-3) / 1e12 / dpeak, "traffic": (tr or {}).get("bytes"), "peak_source": dpeak_src},
-                        "max_rel_dev_tcgen05_vs_dmma": worst}
+                                     "frac": flops / (d_ms * 1e-3) / 1e12 / dpeak, "traffic": None, "peak_source": dpeak_src},
+                        "max_rel_dev_wgmma_vs_dmma": worst}
             except Exception as e:
                 dmma = {"error": str(e)[-200:]}
             finally:
@@ -538,7 +497,7 @@ def run_ours(args):
             return (time.perf_counter() - t0) / k_ * 1e3, k_
 
         e2e_ms, e2e_steps = e2e_time()
-        # the PCIe floor of the step on this box: the same uploads alone
+        # the PCIe floor of the step on this host: the same uploads alone
         t0 = time.perf_counter()
         for _ in range(2):
             dA, dB = s.emptyDataset(), s.emptyDataset()
@@ -581,20 +540,20 @@ def run_ours(args):
         cpu["f2j"] = cpu_f2j_sample(n, blk)
     except Exception as e:  # the secondary baseline must never take the bench line down
         cpu["f2j"] = {"error": str(e)[-300:]}
-    algo_name = ("auto -> Ozaki-II on tcgen05 (int8 residue GEMMs modulo %d coprime moduli%s + CRT; device-side guard, DMMA fallback)"
+    algo_name = ("auto -> Ozaki-II on wgmma (int8 residue GEMMs modulo %d coprime moduli%s + CRT; device-side guard, DMMA fallback)"
                  % (moduli_used, "" if args.crt_moduli else ", count chosen from K: operand truncation 2^-alpha x sqrt(K) <= K 2^-54") if on_tc else "dmma_fp64")
     line = {
         "metric": METRIC, "value": flops / (ms_per_step * 1e-3) / 1e9, "unit": UNIT, "n_gpus": 1,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
-        "config": {"workload": f"{n}x{n} fp64 dense multiply, {blk}-block, 1xB200 (BASELINE metric size)",
+        "config": {"workload": f"{n}x{n} fp64 dense multiply, {blk}-block, 1xH100 (BASELINE metric size)",
                    "inputs": "U(0,1) java.util.Random streams, every block present, column-major",
-                   "l2": f"inputs 2 x {n * n * 8 / 2**30:.0f} GiB + output {n * n * 8 / 2**30:.0f} GiB >> 126 MB L2; no flush needed",
+                   "l2": f"inputs 2 x {n * n * 8 / 2**30:.0f} GiB + output {n * n * 8 / 2**30:.0f} GiB >> 50 MB L2; no flush needed",
                    "gemm_algo": algo_name, "wall_ms_per_step": t_wall / args.steps * 1e3, "c00": checksum,
                    "oz2_ksplit_env": os.environ.get("MATREL_OZ2_KSPLIT")},
         "e2e": {"value": flops / (e2e_ms * 1e-3) / 1e9, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "ms_per_step": e2e_ms, "steps": e2e_steps, "ingest_only_ms": ingest_only_ms,
-                "note": "ingest_only_ms = the step's host->device copies alone on this box: the PCIe floor of the step"},
+                "note": "ingest_only_ms = the step's host->device copies alone on this host: the PCIe floor of the step"},
         "gpu_launches": int(round(launches_per_step * args.steps)),
         "gpu_launches_per_step": launches_per_step,
         "roofline": roofline,
@@ -733,25 +692,25 @@ def run_cfg5(args):
         d2h = sum(v.nbytes for v in outbuf.values()) * world
         s.stop()
     if rank == 0:
-        hbm = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+        hbm = 3350.0                                # NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)
         alg_bytes = (12.0 * nnz_total + 4.0 * (n + nb) * nb + 2 * 8.0 * n * n) / world     # SURVEY 8d compulsory bytes, per rank
-        fma_roof = 148 * 16 * 2 * 1.9e9 / 1e12      # shared-memory port: 16 fp64 FMA / clk / SM at ~1.9 GHz
+        fma_roof = 132 * 16 * 2 * 1.98e9 / 1e12     # shared-memory port: 16 fp64 FMA / clk / SM at the 1.98 GHz maximum clock
         ach_tf = (flops / world) / (kern_ms * 1e-3) / 1e12
         line = {"metric": f"fp64 sparse(1%) x dense block-matmul GFLOP/s at N={n}", "value": flops / (ms * 1e-3) / 1e9, "unit": UNIT,
                 "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "strong",
                 "vs_baseline": None, "dtype": "f64", "data": "synthetic",
-                "config": {"workload": f"BASELINE configs[4]: {n}x{n} sparse(1%) x dense fp64, CSR {blk}-blocks, {plan.pr}x{plan.pc} grid over {world}xB200",
+                "config": {"workload": f"BASELINE configs[4]: {n}x{n} sparse(1%) x dense fp64, CSR {blk}-blocks, {plan.pr}x{plan.pc} grid over {world}xH100",
                            "inputs": "A blocks SparseMatrix.sprand(1024, 1024, 0.01, java.util.Random(1000 + rid*nb + cid)) as CSR, generated on the device; "
                                      "B U(0,1) java.util.Random streams, column-major",
                            "parallelism": "C-stationary grid; sparse block rows replicated where needed (duplicateCrossPartitions), dense B pulled from the grid column over NVLink",
-                           "nnz": nnz_total, "l2": "B panel per rank >> 126 MB L2"},
+                           "nnz": nnz_total, "l2": "B panel per rank >> 50 MB L2"},
                 "e2e": {"value": flops / (e2e_ms * 1e-3) / 1e9, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                         "ms_per_step": e2e_ms, "steps": k_e2e},
                 "gpu_launches": int(st["kernel_launches"] * world), "gpu_launches_per_step_per_rank": st["kernel_launches"] / args.steps,
                 "roofline": {"bound": "hbm", "achieved": alg_bytes / (kern_ms * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s",
                              "frac": alg_bytes / (kern_ms * 1e-3) / 1e9 / hbm, "traffic": None, "kernel": "spmm2_kernel", "kernel_ms": kern_ms,
                              "algorithmic": f"{alg_bytes:.4g} compulsory bytes per rank per launch (12 nnz + 4 (rows + nb) nb + 16 N^2, SURVEY 8d) / world",
-                             "peak_source": "MEASURED_PEAKS.json hbm_gbs",
+                             "peak_source": "NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)",
                              "smem_port": {"achieved_tflops": ach_tf, "roof_tflops": fma_roof, "frac": ach_tf / fma_roof,
                                            "note": "every FMA needs its own 8-byte B element from shared memory: 128 B/clk/SM = 16 FMA/clk/SM is the binding roof"}},
                 "clocks": clocks, "check": {"max_rel_err_vs_host_fp64": err, "blocks_checked": world}}
@@ -772,12 +731,14 @@ def main():
     ap.add_argument("--cpu-budget", type=float, default=15.0)
     ap.add_argument("--ozaki-slices", type=int, default=7)
     ap.add_argument("--algo", type=int, default=0, choices=(0, 1, 2, 4),
-                    help="gemm_algo of the headline: 0 = auto (tcgen05 Ozaki-II with the device-side guard), 1 = DMMA fp64")
+                    help="gemm_algo of the headline: 0 = auto (wgmma Ozaki-II with the device-side guard), 1 = DMMA fp64")
     ap.add_argument("--e2e-chunks", type=int, default=8, help="N > 1: pieces of block rows / block columns the pipelined end-to-end step uploads and pulls")
     ap.add_argument("--crt-moduli", type=int, default=0, help="Ozaki-II residue moduli (6..16); 0 = chosen by the library from K")
     ap.add_argument("--workload", default="metric", choices=("metric", "cfg5"), help="metric = BASELINE metric (dense N=16384); cfg5 = configs[4]")
     ap.add_argument("--n5", type=int, default=32768, help="matrix size of --workload cfg5")
     ap.add_argument("--pull-chunks", type=int, default=4, help="N > 1: pieces the peer pull of A is cut into")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a fixed seeded sample of the last timed step's blocks of C to DIR/*.npy (one GPU, metric workload)")
     ap.add_argument("--_cpu-worker", dest="cpu_worker", default=None, choices=("port", "f2j"), help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.cpu_worker:
@@ -786,6 +747,8 @@ def main():
         if args.impl == "reference":
             print(json.dumps({"impl": "reference", "unavailable": "the reference arm times the metric workload only (dense N=16384)"}))
             return
+        if args.dump_outputs:
+            raise SystemExit("bench.py: --dump-outputs is supported for the metric workload only")
         return run_cfg5(args)
     if args.impl == "reference":
         run_reference(args)

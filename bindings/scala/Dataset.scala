@@ -1,7 +1,7 @@
 /*
  * Scala facade a MatRel maintainer adds next to
  * src/main/scala/org/apache/spark/sql/matfast/Dataset.scala to route the block-multiply path to the
- * B200 engine.  Same method names / argument order as the reference's Dataset (Dataset.scala:38-152);
+ * H100 engine.  Same method names / argument order as the reference's Dataset (Dataset.scala:38-152);
  * each call forwards to the C ABI (include/matrel.h) through the JNI shim (bindings/jni/matrel_jni.cpp).
  * NOT compiled in this image (no scalac / JDK).
  */
@@ -87,7 +87,7 @@ private[b200] object Native {
     }
 }
 
-/** gemmAlgo: 0 = auto (tcgen05 Ozaki-II with the device-side guard, DMMA otherwise), 1 = DMMA fp64 (see matrel.h). */
+/** gemmAlgo: 0 = auto (wgmma Ozaki-II with the device-side guard, DMMA otherwise), 1 = DMMA fp64 (see matrel.h). */
 class B200Session(device: Int = -1, compatBugs: Boolean = true, gemmAlgo: Int = 0) {
   private[b200] val ctx: Long = Native.init(device, compatBugs, gemmAlgo)
   def stop(): Unit = Native.shutdown(ctx)

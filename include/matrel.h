@@ -1,9 +1,9 @@
 /*
- * matrel.h -- C ABI of the B200-native block-matrix engine (drop-in for the MatRel/MatFast
+ * matrel.h -- C ABI of the H100-native block-matrix engine (drop-in for the MatRel/MatFast
  * block-multiply hot path).  Plain C: opaque handles, pointers and sizes; no C++/torch types.
  *
  * Every entry point names the reference interface it replaces.  Paths are relative to
- * /root/reference/src/main/scala/org/apache/spark/sql/matfast/ ("M/").
+ * <reference>/src/main/scala/org/apache/spark/sql/matfast/ ("M/").
  *
  * Conventions
  *   - every function returns mr_status; on failure mr_last_error() (thread-local) holds the
@@ -63,14 +63,14 @@ typedef struct mr_block_desc {
 typedef struct mr_options {
   int32_t device;       /* CUDA device ordinal; -1 = current device */
   int32_t compat_bugs;  /* 1 = reproduce reference defects B3/B4 (SURVEY.md 2.3); 0 = intended math */
-  int32_t gemm_algo;    /* 0 = auto: large regular dense products run on the tcgen05 tensor cores (Ozaki-II: int8 residue GEMMs +
+  int32_t gemm_algo;    /* 0 = auto: large regular dense products run on the int8 tensor cores (Ozaki-II: int8 residue GEMMs +
                            CRT, fp64-exact to 1e-14 on data of ordinary range), guarded on the device: isolated elements more than
                            alpha - 18 binary orders (29 at K = 16384) below the maximum of their row of A / column of B are left out
                            of the residues and their products added exactly in fp64; Inf / NaN operands, more than 64 such elements
                            in one block row / block column, K >= 2^17, irregular block grids and small products take the exact DMMA
                            kernel instead;
                            1 = DMMA fp64 tensor-core kernel (mma.sync m8n8k4 f64), always;
-                           2 = Ozaki-I int8 tcgen05 kernel (digit slices); 3 = 3xTF32 tcgen05 kernel (fp32 results);
+                           2 = Ozaki-I int8 wgmma kernel (digit slices); 3 = 3xTF32 wgmma kernel (fp32 results);
                            4 = Ozaki-II without the range guard.  mr_set_option "crt_moduli": 6..16 residue moduli, 0 (default) = chosen
                               from K so that the operand truncation stays below half the fp64 dot-product bound K 2^-53 (14) */
   int32_t ozaki_slices; /* number of int8 slices for gemm_algo 2 (0 = default) */
@@ -85,7 +85,7 @@ MR_API mr_status mr_init(const mr_options* opts, mr_context** out);
 MR_API mr_status mr_shutdown(mr_context* ctx);
 MR_API mr_status mr_set_stream(mr_context* ctx, void* cuda_stream);
 /* keys: "compat_bugs", "gemm_algo", "ozaki_slices", "crt_moduli", "ozaki_scratch_mb", "spmm_algo", "pipeline", "time_kernels", "gemm_variant",
- *       "oz2_ksplit" (the CTA-pair tcgen05 GEMM walks (modulus, K half, tile pair) work items -- half the L2 footprint of the
+ *       "oz2_ksplit" (the CTA-pair wgmma GEMM walks (modulus, K half, tile pair) work items -- half the L2 footprint of the
  *       residue panels in flight, bit-identical results: 1 = for long tile lists and K >= 8192 only, 2 = whenever possible; default 0,
  *       or the environment variable MATREL_OZ2_KSPLIT at mr_init) */
 MR_API mr_status mr_set_option(mr_context* ctx, const char* key, int64_t value);
@@ -336,11 +336,11 @@ typedef struct mr_stats {
   double last_gemm_ms;      /* CUDA-event duration of the most recent GEMM kernel launch(es) */
   double gemm_ms_total;     /* sum of CUDA-event GEMM durations since reset (timing enabled only) */
   int64_t last_gemm_flops;
-  double tc_gemm_ms_total;  /* CUDA-event time of the tcgen05 int8 GEMM launches since reset (timing enabled only) */
-  int64_t tc_gemm_launches; /* multiplies that ran on the tcgen05 path since reset */
-  int64_t tc_int8_ops;      /* int8 multiply-add operations (x 2) of the most recent tcgen05 multiply */
+  double tc_gemm_ms_total;  /* CUDA-event time of the wgmma int8 GEMM launches since reset (timing enabled only) */
+  int64_t tc_gemm_launches; /* multiplies that ran on the tensor-core path since reset */
+  int64_t tc_int8_ops;      /* int8 multiply-add operations (x 2) of the most recent tensor-core multiply */
   int64_t p2p_bytes;        /* bytes pulled from peer GPUs over NVLink by this context (grid multiply) */
-  int64_t tc_moduli;        /* residue moduli of the most recent tcgen05 (Ozaki-II) multiply */
+  int64_t tc_moduli;        /* residue moduli of the most recent tensor-core (Ozaki-II) multiply */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

@@ -1,6 +1,6 @@
 // matrel.hpp -- header-only C++17 mirror of the reference's Dataset operator API over the C ABI
 // (include/matrel.h).  Method names and argument order follow
-// /root/reference/src/main/scala/org/apache/spark/sql/matfast/Dataset.scala:57-152; `require`
+// <reference>/src/main/scala/org/apache/spark/sql/matfast/Dataset.scala:57-152; `require`
 // failures surface as matfast::IllegalArgumentException carrying the reference's message text.
 #pragma once
 #include <cstdint>

@@ -1,7 +1,7 @@
-"""matrel_b200 -- B200-native block-matrix engine behind the MatRel/MatFast Dataset operator API.
+"""matrel_b200 -- H100-native block-matrix engine behind the MatRel/MatFast Dataset operator API.
 
 Layout (only what the block-multiply hot path needs):
-  csrc/            sm_100a CUDA kernels + the C-ABI host layer (include/matrel.h)
+  csrc/            sm_90a CUDA kernels + the C-ABI host layer (include/matrel.h)
   _native.py       ctypes binding of the C ABI (fails loudly when the .so is missing)
   matrix.py        DenseMatrix / SparseMatrix / MatrixBlock containers (reference data model)
   dataset.py       MatfastSession + Dataset: the reference's operator names and argument order

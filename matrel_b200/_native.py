@@ -185,7 +185,7 @@ _STR_FUNCS = ("mr_last_error", "mr_version")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(nvcc, sm_100a). matrel_b200 has no CPU fallback.")
+        "(nvcc, sm_90a). matrel_b200 has no CPU fallback.")
 
 lib = C.CDLL(LIB_PATH)
 for _name, _args in SIGNATURES.items():

@@ -1,4 +1,4 @@
-// C-ABI host layer of the B200 block-matrix engine (see include/matrel.h): context lifetime, device memory, block ingest /
+// C-ABI host layer of the H100 block-matrix engine (see include/matrel.h): context lifetime, device memory, block ingest /
 // egress and the helpers shared by the operator files (abi_multiply.cpp, abi_elementwise.cpp, abi_aggregate.cpp,
 // abi_partition.cpp).
 //
@@ -265,7 +265,7 @@ Span upload_raw(mr_context* ctx, const void* host, size_t bytes) {
 extern "C" {
 
 const char* mr_last_error(void) { return g_last_error.c_str(); }
-const char* mr_version(void) { return "matrel-b200 0.1 (sm_100a)"; }
+const char* mr_version(void) { return "matrel-b200 0.1 (sm_90a)"; }
 
 mr_status mr_init(const mr_options* opts, mr_context** out) {
   return guarded([&] {
@@ -274,7 +274,7 @@ mr_status mr_init(const mr_options* opts, mr_context** out) {
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0) {
       (void)cudaGetLastError();
-      fail(MR_ECUDA, "no usable CUDA device (%s): the B200 engine has no CPU fallback",
+      fail(MR_ECUDA, "no usable CUDA device (%s): the engine has no CPU fallback",
            e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
     }
     auto ctx = std::unique_ptr<mr_context>(new mr_context);
@@ -285,8 +285,8 @@ mr_status mr_init(const mr_options* opts, mr_context** out) {
     ctx->device = dev;
     cudaDeviceProp prop{};
     CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 10)
-      fail(MR_ECUDA, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", dev, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+      fail(MR_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", dev, prop.major, prop.minor);
     if (opts) {
       ctx->compat_bugs = opts->compat_bugs;
       ctx->gemm_algo = opts->gemm_algo;

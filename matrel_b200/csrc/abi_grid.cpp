@@ -1,7 +1,7 @@
 // Multi-GPU layer of the C ABI: datasets sharded over a pr x pc process grid, the grid multiply, and the single-process grid
 // (one process drives all GPUs of the box).
 //
-// What it replaces in the reference (M/ = /root/reference/src/main/scala/org/apache/spark/sql/matfast/):
+// What it replaces in the reference (M/ = <reference>/src/main/scala/org/apache/spark/sql/matfast/):
 //   * RowPartitioner / ColumnPartitioner placement (M/partitioner/RowPartitioner.scala:34, ColumnPartitioner.scala:34): rank (r, c)
 //     owns the blocks with rid % pr == r and cid % pc == c -- of A, B and C alike (C-stationary);
 //   * the two groupByKey + join of matrixMultiplyGeneral (M/execution/MatfastExecutionHelper.scala:236-249) that co-locate A(:, k)
@@ -731,7 +731,7 @@ mr_status mr_init_grid(const mr_options* opts, int32_t ngpus, mr_grid** out) {
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
       (void)cudaGetLastError();
-      fail(MR_ECUDA, "no usable CUDA device: the B200 engine has no CPU fallback");
+      fail(MR_ECUDA, "no usable CUDA device: the engine has no CPU fallback");
     }
     MR_REQUIRE(ngpus <= count, MR_EINVAL, "grid of %d GPUs requested, %d visible", ngpus, count);
     std::unique_ptr<mr_grid> g(new mr_grid);

@@ -1,5 +1,5 @@
 // Block multiply: planning (LocalMatrix.matrixMultiplication dispatch), the fused DMMA launch incl. the pipelined chunks,
-// the tcgen05 paths, sparse x dense and sparse x sparse partial products, and the mr_matrix_multiply entry point.
+// the wgmma paths, sparse x dense and sparse x sparse partial products, and the mr_matrix_multiply entry point.
 #include "host.h"
 
 using namespace matrel;
@@ -89,7 +89,7 @@ struct MultiplyPlanner {
   }
 };
 
-// gemm_algo 2: the dense pairs of every output block through the tcgen05 int8 Ozaki pipeline (gemm_ozaki.cu).
+// gemm_algo 2: the dense pairs of every output block through the wgmma int8 Ozaki pipeline (gemm_ozaki.cu).
 // Returns false when the problem does not fit its regular-grid assumptions or holds Inf/NaN (caller uses DMMA).
 bool try_ozaki(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<double*>& cptr, int32_t blkSize, int64_t M,
                int64_t K, int64_t N, bool outer) {
@@ -318,7 +318,7 @@ struct Oz2Run {
       }
       return runs;
     };
-    // slots that start on even 128-row tiles let the cta_group::2 kernel run the tiles in vertically adjacent pairs
+    // slots that start on even 128-row tiles let the CTA-pair kernel run the tiles in vertically adjacent pairs
     const bool paired = (ss % (2 * kOz2TileM)) == 0 && ctx->force_variant != 2;
     auto add_tiles = [&](Job& j, int rslot, int cslot, int m, int n) {
       const int tm0 = rslot * ss / kOz2TileM;
@@ -691,7 +691,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
         wait_ready(ctx, *g.b);
       }
   };
-  // gemm_algo: 0 = auto (Ozaki-II on tcgen05 with the range guard when the product is large and regular, else DMMA), 1 = DMMA,
+  // gemm_algo: 0 = auto (Ozaki-II on wgmma with the range guard when the product is large and regular, else DMMA), 1 = DMMA,
   // 2 = Ozaki-I, 3 = 3xTF32, 4 = Ozaki-II without the range guard
   const int algo = ctx->gemm_algo;
   bool ozaki_done = false;
@@ -701,10 +701,10 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     if (ozaki_done) ctx->stats.last_gemm_flops = flops;
   }
   if (!outs.empty() && !ozaki_done) {
-    // tile shape: large tiles unless they cannot fill the 148 SMs
+    // tile shape: large tiles unless they cannot fill the 132 SMs
     int64_t tiles128 = 0;
     for (auto& go : outs) tiles128 += static_cast<int64_t>((go.m + 127) / 128) * ((go.n + 127) / 128);
-    int variant = tiles128 >= 2 * 148 ? GEMM_128x128 : GEMM_64x64;
+    int variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
     if (ctx->force_variant >= 0) variant = ctx->force_variant;
     const int BM = gemm_tile_m(variant), BN = gemm_tile_n(variant);
     const int tpbm = std::max(1, (blkSize + BM - 1) / BM), tpbn = std::max(1, (blkSize + BN - 1) / BN);
@@ -713,7 +713,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       GemmTile t;
     };
     std::vector<Keyed> keyed;
-    constexpr int kBand = 12;  // ~12 x 12 tiles resident across 148 SMs share A row- and B column-panels in L2
+    constexpr int kBand = 12;  // the ~132 resident tiles (12 columns x 11 rows) share A row- and B column-panels in L2; carried over, not re-tuned for H100
     for (size_t oi = 0; oi < outs.size(); ++oi) {
       const OutPlan& o = plans[out_plan[oi]];
       const int tm = (outs[oi].m + BM - 1) / BM, tn = (outs[oi].n + BN - 1) / BN;
@@ -745,7 +745,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
         order[oi] = {key, oi};
       }
       std::sort(order.begin(), order.end());
-      const int64_t min_tiles = 148;  // >= one wave; the launches overlap on the side streams, so small chunks cost nothing
+      const int64_t min_tiles = 132;  // >= one wave; the launches overlap on the side streams, so small chunks cost nothing
       int64_t acc_tiles = 0;
       int gcur = 0;
       for (size_t r = 0; r < order.size(); ++r) {
@@ -760,7 +760,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       }
       ngroups_dyn = gcur + 1;
     }
-    // The tcgen05 path (Ozaki-II residues + CRT) runs group by group in front of the DMMA launches, which then only execute
+    // The int8 tensor-core path (Ozaki-II residues + CRT) runs group by group in front of the DMMA launches, which then only execute
     // when the engine's device flag reports operands it cannot represent.  Small products stay on the exact kernel in auto mode.
     Oz2Run oz2;
     bool use_oz2 = false;
@@ -817,7 +817,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     for (int gi = 0; gi < ngroups; ++gi) {
       size_t t1 = t0;
       while (t1 < keyed.size() && grp(keyed[t1]) == gi) ++t1;
-      // DMMA chunks are independent launches: round-robin over the side streams so that tails overlap.  The tcgen05 engine's
+      // DMMA chunks are independent launches: round-robin over the side streams so that tails overlap.  The Ozaki-II engine's
       // jobs share its residue planes and each fills the machine by itself (persistent kernel): one side stream, in order.
       cudaStream_t cs = side ? ctx->chunk_stream[use_oz2 ? 0 : gi % mr_context::kChunkStreams] : ctx->stream;
       // wait for exactly the operand blocks this chunk reads

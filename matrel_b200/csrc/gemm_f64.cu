@@ -1,12 +1,12 @@
-// fp64 block-GEMM for sm_100a: C(i,j) = sum_k A(i,k) * B(k,j) over the present k-blocks.
+// fp64 block-GEMM for sm_90a: C(i,j) = sum_k A(i,k) * B(k,j) over the present k-blocks.
 //
 // Replaces, in one kernel launch per matrixMultiply call:
 //   - BLAS.gemmddd -> nativeBLAS.dgemm per block pair   (M/matrix/BLAS.scala:327-346)
 //   - MLMatrix.multiply's fresh zeroed C per pair       (M/matrix/MLMatrix.scala:100-104)
 //   - reduceByKey(LocalMatrix.add) over k               (M/execution/MatfastExecutionHelper.scala:255)
 //
-// Design (B200 has no fp64 kind in tcgen05; the fp64 tensor pipe is reached through
-// mma.sync.m8n8k4.f64 = SASS DMMA.8x8x4, measured 37.07 TFLOP/s, profiles/fp64_peaks_r01.jsonl):
+// Design (wgmma has no fp64 kind; the fp64 tensor pipe is reached through
+// mma.sync.m8n8k4.f64 = SASS DMMA):
 //   - warp-specialised CTA: 1 producer warp + NCW consumer warps, STAGES-deep shared-memory ring,
 //     full/empty mbarriers per stage; consumers keep the whole K reduction (all k-blocks of the
 //     block row/column) in registers.

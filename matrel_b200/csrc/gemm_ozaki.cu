@@ -1,6 +1,6 @@
-// fp64 block-GEMM on the 5th-generation tensor cores (tcgen05, kind::i8) through Ozaki splitting.
+// fp64 block-GEMM on the Hopper tensor cores (wgmma, s8 x s8 -> s32) through Ozaki splitting.
 //
-// tcgen05.mma has no fp64 kind, so the north-star's "block multiply as tcgen05 tiles" is only reachable for
+// wgmma has no fp64 kind, so the north-star's "block multiply as tensor-core tiles" is only reachable for
 // fp64 data by error-free integer slicing (Ozaki scheme I, the technique behind vendor "fp64 emulation"):
 //   a_ik = 2^(e_i+2) * sum_{s=1..S} A_s[i,k] * 2^(-8s)      A_s in [-128,127]  (balanced base-256 digits, |a_ik| < 2^e_i)
 //   b_kj = 2^(f_j+2) * sum_{t=1..S} B_t[k,j] * 2^(-8t)
@@ -15,9 +15,9 @@
 // MLMatrix.scala:100-104, MatfastExecutionHelper.scala:255):
 //   1. absmax pass over the blocks of A (per global row) and B (per global column)      -- HBM-bound
 //   2. slice pass: S int8 matrices A_s [M x K] and B_t^T [N x K], K contiguous            -- HBM-bound
-//   3. for each diagonal d: ONE tcgen05 GEMM launch: TMA (SWIZZLE_128B tensor maps) -> 4-stage smem ring ->
-//      tcgen05.mma.kind::i8 (one elected thread, 128x256 s32 accumulator in TMEM) over all (s, d-s) pairs and
-//      all k -> tcgen05.ld epilogue: scale by 2^(e_i+f_j+4-8d) and accumulate into the fp64 output blocks.
+//   3. for each diagonal d: ONE GEMM launch: TMA (SWIZZLE_128B tensor maps) -> 4-stage smem ring ->
+//      wgmma m64n256k32 s8 (two consumer warpgroups, 64 x 256 s32 accumulator in registers each) over all (s, d-s)
+//      pairs and all k -> register epilogue: scale by 2^(e_i+f_j+4-8d) and accumulate into the fp64 output blocks.
 #include <cuda.h>
 
 #include <algorithm>
@@ -25,6 +25,7 @@
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "kernels.h"
@@ -32,10 +33,8 @@
 namespace matrel {
 namespace {
 
-constexpr int BM = 128, BN = 256, BKB = 128 /* bytes (= int8 elements) of K per stage */, UMMA_K = 32, STAGES = 4;
+constexpr int BM = 128, BN = 256, BKB = 128 /* bytes (= int8 elements) of K per stage */, WGMMA_KB = 32 /* bytes of K per wgmma */, STAGES = 4;
 constexpr int A_BYTES = BM * BKB, B_BYTES = BN * BKB, STAGE_BYTES = A_BYTES + B_BYTES;
-
-
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -59,29 +58,43 @@ __device__ __forceinline__ void tma_2d(uint32_t dst, const void* tmap, int c0, i
                "l"(tmap), "r"(bar), "r"(c0), "r"(c1)
                : "memory");
 }
-// UMMA shared-memory descriptor, K-major operand tile, SWIZZLE_128B: rows of 128 B, 8-row groups 1024 B apart
-// (start >> 4 @ [0,14), LBO = 1 @ [16,30), SBO = 1024 >> 4 @ [32,46), version 1 @ [46,48), layout SWIZZLE_128B = 2 @ [61,64))
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr) {
-  return static_cast<uint64_t>((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// wgmma shared-memory descriptor, K-major operand tile, SWIZZLE_128B: rows of 128 B, 8-row groups 1024 B apart
+// (start >> 4 @ [0,14), LBO = 1 @ [16,30) (unused by swizzled K-major tiles), SBO = 1024 >> 4 @ [32,46), SWIZZLE_128B = 1 @ [62,64))
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t saddr) {
+  return static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void umma_i8(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_c),
-               "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-               : "memory");
+#define WG_OPS16(c, a, o)                                                                                                          \
+  c(a[o]), c(a[o + 1]), c(a[o + 2]), c(a[o + 3]), c(a[o + 4]), c(a[o + 5]), c(a[o + 6]), c(a[o + 7]), c(a[o + 8]), c(a[o + 9]),    \
+      c(a[o + 10]), c(a[o + 11]), c(a[o + 12]), c(a[o + 13]), c(a[o + 14]), c(a[o + 15])
+#define WG_OPS128(c, a)                                                                                                            \
+  WG_OPS16(c, a, 0), WG_OPS16(c, a, 16), WG_OPS16(c, a, 32), WG_OPS16(c, a, 48), WG_OPS16(c, a, 64), WG_OPS16(c, a, 80),           \
+      WG_OPS16(c, a, 96), WG_OPS16(c, a, 112)
+#define WG_D128                                                                                                                    \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "     \
+  "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, " \
+  "%51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, " \
+  "%76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, " \
+  "%101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, "       \
+  "%121, %122, %123, %124, %125, %126, %127}"
+// D (64 x 256, this warpgroup's registers) (+)= A (64 x 32 bytes of K) * B (256 x 32 bytes of K), both from shared memory
+__device__ __forceinline__ void wgmma_tile(int32_t (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\twgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 " WG_D128
+               ", %128, %129, p;\n\t}"
+               : WG_OPS128("+r", d)
+               : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_c),
-               "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-               : "memory");
+__device__ __forceinline__ void wgmma_tile(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\twgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 " WG_D128
+               ", %128, %129, p, 1, 1;\n\t}"
+               : WG_OPS128("+f", d)
+               : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-#define TMEM_LD16(taddr, r)                                                                                             \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"   \
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), \
-                 "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])                  \
-               : "r"(taddr))
 
 struct OzakiGemmParams {
   const unsigned char* tmaps;  // 2*S CUtensorMaps (128 B each): A_1..A_S then B_1..B_S
@@ -94,13 +107,11 @@ struct OzakiGemmParams {
   int32_t accumulate;          // 0: C = term, 1: C += term
   int32_t tiles_m, tiles_n;    // tile grid (128 x 256 tiles)
   double diag_scale;           // 2^(4 - 8 d)
-  // generalisation used by the fp32 path (tf32x3): explicit (A slice, B slice) tensor-map index pairs, the K extent of
-  // one 128-byte stage row in elements, the UMMA instruction descriptor and the accumulator type
+  // generalisation used by the fp32 path (tf32x3): explicit (A slice, B slice) tensor-map index pairs and the K extent of
+  // one 128-byte stage row in elements (the accumulator type is the kernel's template parameter)
   int32_t npairs;
   int32_t pair_a[8], pair_b[8];
   int32_t kstep;               // elements of K per stage (128 int8 / 32 tf32)
-  uint32_t idesc;
-  int32_t f32_acc;             // 0: s32 accumulator scaled by the Ozaki exponents; 1: f32 accumulator written as is
   int32_t kc0, nkc;            // K range of this launch in stage units (the fp32 path re-accumulates K chunks in fp64)
   // CRT mode (Ozaki scheme II, gemm_algo 4): nmod > 0 makes ONE launch walk nmod x tiles work items; item (t, tile) multiplies
   // residue matrices A mod p_t (tensor map t) and B mod p_t (tensor map nmod + t) and stores (A_t B_t) mod p_t as int8.
@@ -117,10 +128,15 @@ struct OzakiGemmParams {
   const int* gate;
 };
 
-constexpr int EPI_WARPS = 8;                       // 2 per TMEM lane quarter (each takes 128 of the 256 columns)
-constexpr int GEMM_THREADS_P = (4 + EPI_WARPS) * 32;
-constexpr int TMEM_COLS_P = 512;                   // two 128 x 256 s32 accumulators: MMA of tile i+1 overlaps epilogue of tile i
+// warpgroup 0: TMA producer (one elected thread); warpgroups 1, 2: wgmma consumers, 64 of the tile's 128 rows each, and epilogue
+constexpr int CONSUMER_WARPS = 8;
+constexpr int GEMM_THREADS_P = 128 + CONSUMER_WARPS * 32;
+constexpr size_t GEMM_SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 2 * STAGES * 8;  // alignment slack, ring, full[] + empty[] barriers
 constexpr int TILE_BAND = 8;                       // n-tiles per rasterisation band (L2 reuse of A / B panels)
+
+// 384 threads x 168 registers fill the register file: the producer warpgroup hands its share to the two accumulator holders
+__device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
 __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int& tm, int& tn) {
   const int band_tiles = TILE_BAND * tiles_m;
@@ -131,14 +147,66 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   tn = band * TILE_BAND + rem % bw;
 }
 
-// Persistent, warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator,
-// warps 4..11 = epilogue.  One CTA per SM loops over the output tiles of this diagonal.
+// The wgmma accumulator fragment: thread (warp wq of the warpgroup, lane) holds, for every 8-column group j = 0..31,
+// acc[4 j + e] = element (16 wq + lane / 4 + 8 (e >> 1), 8 j + 2 (lane % 4) + (e & 1)) of the warpgroup's 64 x 256 tile.
+
+// K loop of one work item in a consumer warpgroup: `steps` ring stages accumulate into acc (the first overwrites it).  One
+// stage's wgmmas stay in flight while the next stage is awaited; every warp hands a stage back once its wgmmas have retired.
+template <class Acc, class Release>
+__device__ __forceinline__ void consume_item(Acc (&acc)[128], unsigned char* smem, uint64_t* bars, int a_off, int steps, int& it, int lane,
+                                             Release&& release) {
+  wgmma_fence();
+  for (int j = 0; j < steps; ++j, ++it) {
+    const int st = it % STAGES;
+    mbar_wait(smem_u32(&bars[st]), (it / STAGES) & 1);
+    const uint32_t a0 = smem_u32(smem + st * STAGE_BYTES) + a_off, b0 = smem_u32(smem + st * STAGE_BYTES) + A_BYTES;
+#pragma unroll
+    for (int k = 0; k < BKB / WGMMA_KB; ++k)  // 4 wgmmas of 32 bytes of K each (32 int8 / 8 tf32)
+      wgmma_tile(acc, wgmma_desc_k_sw128(a0 + k * WGMMA_KB), wgmma_desc_k_sw128(b0 + k * WGMMA_KB), (j | k) != 0);
+    wgmma_commit();
+    if (j > 0) {
+      wgmma_wait<1>();
+      if (lane == 0) release((it - 1) % STAGES);
+    }
+  }
+  wgmma_wait<0>();
+  if (lane == 0) release((it - 1) % STAGES);
+}
+
+// Residues of a warpgroup's exact s32 accumulator into the compact plane of its tile ([128 rows][256 columns] bytes).
+// q = rint(c / p) is exact in fp64 (no integer c / p lies within 1/(2p) of a tie except the true ties of the even modulus 256,
+// where either neighbour is a valid representative).  ADD: the residue byte this SAME thread stored for the lower K half joins
+// the sum before the reduction: ((x mod p) + y) mod p = (x + y) mod p; |y| <= K/2 * 2^14 and x < 256 keep the sum inside int32.
+template <bool ADD>
+__device__ __forceinline__ void store_residues(const int32_t (&acc)[128], int8_t* tile, int row, int lane, int pm, double pinv) {
+  int8_t* dst = tile + static_cast<size_t>(row) * BN + 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint16_t* d2 = reinterpret_cast<uint16_t*>(dst + h * 8 * BN + 8 * j);
+      const uint32_t prev = ADD ? *d2 : 0u;
+      uint32_t wv = 0;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        int v = acc[4 * j + 2 * h + e];
+        if (ADD) v += static_cast<int>((prev >> (8 * e)) & 0xffu);
+        int res = v - __double2int_rn(static_cast<double>(v) * pinv) * pm;  // [-p/2, p/2]
+        res += (res >> 31) & pm;                                          // [0, p): the CRT kernel reads unsigned bytes
+        wv |= static_cast<uint32_t>(res) << (8 * e);
+      }
+      *d2 = static_cast<uint16_t>(wv);
+    }
+  }
+}
+
+// Persistent, warp-specialised: one CTA per SM loops over the output tiles of this launch.  F32 = false: s8 operands, exact s32
+// accumulator (Ozaki slices or CRT residues); F32 = true: tf32 operands, fp32 accumulator written as is (tf32x3_gemm).
+template <bool F32>
 __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const OzakiGemmParams p) {
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  // barriers: full[STAGES], empty[STAGES], acc_full[2], acc_empty[2]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);  // full[STAGES], empty[STAGES]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (p.gate != nullptr && *p.gate != 0) return;  // uniform: non-finite / out-of-range operands take the exact DMMA kernel
   const int nk = p.nkc;
@@ -148,27 +216,17 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bars[s]), 1);
-      mbar_init(smem_u32(&bars[STAGES + s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&bars[2 * STAGES + b]), 1);              // acc_full: one tcgen05.commit
-      mbar_init(smem_u32(&bars[2 * STAGES + 2 + b]), EPI_WARPS);  // acc_empty: one arrival per epilogue warp
+      mbar_init(smem_u32(&bars[s]), 1);                        // full: the producer's arrive.expect_tx
+      mbar_init(smem_u32(&bars[STAGES + s]), CONSUMER_WARPS);  // empty: one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS_P) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
+    producer_regs();
     // ===== TMA producer (one elected lane) =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int it = 0;
       for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
         const int mi = w / ntiles, t = w - mi * ntiles;
@@ -196,41 +254,14 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one elected lane): every (s, d-s) pair and every k accumulates into one s32 tile =====
-    if (lane == 0) {
-      const uint32_t idesc = p.idesc;
-      int it = 0, lt = 0;
-      for (int w = blockIdx.x; w < nitems; w += gridDim.x, ++lt) {
-        const int buf = lt & 1;
-        const uint32_t aph = (lt >> 1) & 1;
-        mbar_wait(smem_u32(&bars[2 * STAGES + 2 + buf]), aph ^ 1);  // epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + static_cast<uint32_t>(buf * BN);
-        for (int j = 0; j < per_tile; ++j, ++it) {
-          const int st = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(smem_u32(&bars[st]), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a0 = smem_u32(smem + st * STAGE_BYTES), b0 = a0 + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BKB / UMMA_K; ++k) {  // 4 MMAs of 32 bytes of K each (32 int8 / 8 tf32)
-            const uint64_t da = umma_desc_k_sw128(a0 + k * UMMA_K), db = umma_desc_k_sw128(b0 + k * UMMA_K);
-            if (p.f32_acc) umma_tf32(tacc, da, db, idesc, (j | k) != 0);
-            else umma_i8(tacc, da, db, idesc, (j | k) != 0);
-          }
-          umma_commit(smem_u32(&bars[STAGES + st]));  // stage is free once these MMAs retire
-        }
-        umma_commit(smem_u32(&bars[2 * STAGES + buf]));  // accumulator complete
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: TMEM -> registers -> scale by 2^(e_i + f_j + 4 - 8d) -> (+)= column-major fp64 output blocks =====
-    const int ew = warp - 4;
-    const int q = ew & 3;          // TMEM lane quarter this warp may access (warp id % 4)
-    const int half = ew >> 2;      // which 128 of the tile's 256 columns
-    int lt = 0;
-    for (int w = blockIdx.x; w < nitems; w += gridDim.x, ++lt) {
+  } else {
+    consumer_regs();
+    // ===== consumers: every (s, d-s) pair and every k accumulates into one register tile, then the epilogue =====
+    const int cw = (warp - 4) >> 2, wq = warp & 3;  // consumer warpgroup, warp within it
+    const int trow = 64 * cw + 16 * wq + (lane >> 2);  // first of this thread's two tile rows (the other is trow + 8)
+    typename std::conditional<F32, float, int32_t>::type acc[128];
+    int it = 0;
+    for (int w = blockIdx.x; w < nitems; w += gridDim.x) {
       const int mi = w / ntiles, t = w - mi * ntiles;
       int tm, tn;
       if (p.tile_list) {
@@ -240,114 +271,63 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
       } else {
         tile_coords(t, p.tiles_m, p.tiles_n, tm, tn);
       }
-      const int m0 = tm * BM, n0 = tn * BN;
-      const int buf = lt & 1;
-      const uint32_t aph = (lt >> 1) & 1;
-      const int row = m0 + q * 32 + lane;
-      const bool row_ok = row < p.M;
-      const int rid = row_ok ? row / p.blk : 0;
-      const int lr = row - rid * p.blk;
-      const int brows = min(p.blk, p.M - rid * p.blk);
-      const double rs = (p.f32_acc || p.nmod) ? 1.0 : (row_ok ? p.row_scale[row] * p.diag_scale : 0.0);
-      // fp32 path: the fp64 mean corrections go in with the first K chunk (see slice_tf32_kernel)
-      const bool f32_corr = p.f32_acc && !p.accumulate && p.row_scale != nullptr;
-      const double rcorr = (f32_corr && row_ok) ? p.row_scale[row] : 0.0;
-      mbar_wait(smem_u32(&bars[2 * STAGES + buf]), aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tsrc = tmem_base + static_cast<uint32_t>(buf * BN) + (static_cast<uint32_t>(q * 32) << 16) + half * 128;
-#pragma unroll 1
-      for (int c = 0; c < 128; c += 16) {
-        uint32_t r[16];
-        TMEM_LD16(tsrc + c, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (c == 128 - 16) {
-          // all of this warp's accumulator reads are in registers: hand the buffer back to the MMA warp
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&bars[2 * STAGES + 2 + buf]));
-        }
-        const int col0 = n0 + half * 128 + c;
+      consume_item(acc, smem, bars, cw * 64 * BKB, per_tile, it, lane, [&](int st) { mbar_arrive(smem_u32(&bars[STAGES + st])); });
+      if constexpr (!F32) {
         if (p.nmod) {
-          // residue of the exact s32 dot product: q = rint(c / p) is exact in fp64 (no integer c / p lies within 1/(2p) of a
-          // tie except the true ties of the even modulus 256, where either neighbour is a valid representative)
-          const int pm = p.mod_p[mi];
-          const double pinv = p.mod_inv[mi];
-          uint32_t packed[4];
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint32_t wv = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int v = static_cast<int32_t>(r[4 * g + j]);
-              int res = v - __double2int_rn(static_cast<double>(v) * pinv) * pm;  // [-p/2, p/2]
-              res += (res >> 31) & pm;                                          // [0, p): the CRT kernel reads unsigned bytes
-              wv |= static_cast<uint32_t>(res) << (8 * j);
-            }
-            packed[g] = wv;
-          }
           // compact planes: [modulus][tile of this launch][128 rows][256 columns], always whole tiles (no guards)
-          int8_t* dst = p.planes + static_cast<size_t>(mi) * p.plane_stride + static_cast<size_t>(t) * (BM * BN) +
-                        static_cast<size_t>(q * 32 + lane) * BN + half * 128 + c;
-          *reinterpret_cast<uint4*>(dst) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-        } else if (row_ok && col0 < p.N) {
-          const int cid0 = col0 / p.blk;
-          const bool one_block = (col0 + 15 < p.N) && ((col0 + 15) / p.blk == cid0);
-          if (one_block) {
-            double* blkp = p.ctab[rid * p.nbc + cid0];
+          store_residues<false>(acc, p.planes + static_cast<size_t>(mi) * p.plane_stride + static_cast<size_t>(t) * (BM * BN), trow, lane,
+                                p.mod_p[mi], p.mod_inv[mi]);
+          continue;
+        }
+      }
+      // scale by 2^(e_i + f_j + 4 - 8d) (s32) or take as is (fp32) -> (+)= column-major fp64 output blocks
+      // fp32 path: the fp64 mean corrections go in with the first K chunk (see slice_tf32_kernel)
+      const bool f32_corr = F32 && !p.accumulate && p.row_scale != nullptr;
+      bool row_ok[2];
+      int rid[2], lr[2], brows[2];
+      double rs[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = tm * BM + trow + 8 * h;
+        row_ok[h] = row < p.M;
+        rid[h] = row_ok[h] ? row / p.blk : 0;
+        lr[h] = row - rid[h] * p.blk;
+        brows[h] = min(p.blk, p.M - rid[h] * p.blk);
+        rs[h] = !row_ok[h] ? 0.0 : (F32 ? (f32_corr ? p.row_scale[row] : 0.0) : p.row_scale[row] * p.diag_scale);
+      }
+      const int col0 = tn * BN + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int h = e >> 1, col = col0 + 8 * j + (e & 1);
+          if (row_ok[h] && col < p.N) {
+            const int cid = col / p.blk;
+            double* blkp = p.ctab[rid[h] * p.nbc + cid];
             if (blkp != nullptr) {
-              double* dst = blkp + lr + static_cast<size_t>(brows) * (col0 - cid0 * p.blk);
-              double old[16];
-              if (p.accumulate) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) old[j] = dst[static_cast<size_t>(brows) * j];
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) old[j] = 0.0;
-              }
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                dst[static_cast<size_t>(brows) * j] =
-                    p.f32_acc ? old[j] + static_cast<double>(__uint_as_float(r[j])) + (f32_corr ? rcorr + __ldg(p.col_scale + col0 + j) : 0.0)
-                              : old[j] + (static_cast<double>(static_cast<int32_t>(r[j])) * rs) * __ldg(p.col_scale + col0 + j);
-            }
-          } else {
-#pragma unroll 1
-            for (int j = 0; j < 16; ++j) {
-              const int col = col0 + j;
-              if (col < p.N) {
-                const int cid = col / p.blk;
-                double* blkp = p.ctab[rid * p.nbc + cid];
-                if (blkp != nullptr) {
-                  double* dst = blkp + lr + static_cast<size_t>(brows) * (col - cid * p.blk);
-                  const double term = p.f32_acc ? static_cast<double>(__uint_as_float(r[j])) + (f32_corr ? rcorr + p.col_scale[col] : 0.0)
-                                                : (static_cast<double>(static_cast<int32_t>(r[j])) * rs) * p.col_scale[col];
-                  *dst = p.accumulate ? *dst + term : term;
-                }
-              }
+              double* dst = blkp + lr[h] + static_cast<size_t>(brows[h]) * (col - cid * p.blk);
+              double term;
+              if constexpr (F32) term = static_cast<double>(acc[4 * j + e]) + (f32_corr ? rs[h] + __ldg(p.col_scale + col) : 0.0);
+              else term = (static_cast<double>(acc[4 * j + e]) * rs[h]) * __ldg(p.col_scale + col);
+              *dst = p.accumulate ? *dst + term : term;
             }
           }
         }
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS_P) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------
-// The same residue GEMM on CTA PAIRS (tcgen05 cta_group::2): a cluster of two CTAs (the two SMs of a TPC) computes a 256 x 256
-// tile.  Each CTA stages ITS 128 rows of A' and ITS 128 columns (rows of the K-major B') of the tile -- 32 KB per stage instead
-// of 48 KB -- and the pair's tensor cores share them, so per k-byte an SM writes 256 B and reads 256 B of shared memory instead
-// of 384 + 384: at kind::i8 rates the single-CTA kernel is bound by exactly that (ncu: tensor pipe 67 % = 128 / 192 of the
-// 128 B/clk shared-memory port).  Roles per CTA: warp 0 TMA producer (own halves; completion is signalled on the LEADER's full
-// barrier), warp 1 of the leader issues the M = 256 MMAs for both, warp 2 TMEM allocator (two 128 x 256 s32 accumulators per
-// CTA), warps 4..11 epilogue (own 128 rows -> residues -> compact planes).  Only used by the Ozaki-II engine: work item =
-// (modulus, pair of vertically adjacent 128-row tiles); the tile list holds the two halves at positions 2 t and 2 t + 1.
+// The same residue GEMM on CTA PAIRS: a cluster of two CTAs computes a 256 x 256 tile, each CTA its own 128 rows.  Both need the
+// same 256 columns (rows of the K-major B'), so each CTA fetches only HALF of them and multicasts that half into the shared
+// memory of both (TMA .multicast::cluster): per stage a CTA requests 16 KB of A' and 16 KB of B' from L2 instead of 16 + 32,
+// which is what the persistent kernel runs short of once the CTAs in flight have drifted apart in k.  Roles per CTA as in the
+// single-CTA kernel; a stage is free for the pair's producers once the consumer warps of BOTH CTAs have released it, so the empty
+// barriers count the arrivals of the whole pair.  Only used by the Ozaki-II engine: work item = (modulus, pair of vertically
+// adjacent 128-row tiles); the tile list holds the two halves at positions 2 t and 2 t + 1.
 // ------------------------------------------------------------------------------------------------
-constexpr int STAGES2 = 6;
-constexpr int B2_BYTES = (BN / 2) * BKB, STAGE2_BYTES = A_BYTES + B2_BYTES;
-constexpr size_t SMEM2_BYTES = 1024 + STAGES2 * STAGE2_BYTES + (2 * STAGES2 + 4) * 8 + 16;
+constexpr int B2_BYTES = (BN / 2) * BKB;
 
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
   uint32_t r;
@@ -357,16 +337,22 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank)
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
+// the box lands at the same shared-memory offset, and completes the barrier at the same offset, in every CTA of the mask
+__device__ __forceinline__ void tma_2d_multicast(uint32_t dst, const void* tmap, int c0, int c1, uint32_t bar, uint16_t cta_mask) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+               ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
+               : "memory");
+}
 
-// The work items of ONE CTA pair in execution order; the producer, the MMA issuer and the epilogue warps walk identical copies.
+// The work items of ONE CTA pair in execution order; the producers and the consumer warps of both CTAs walk identical copies.
 //   KSPLIT = false: item = (modulus, tile pair), flat index w = cl, cl + ncl, ... over nmod x npairs, the whole K per item.
 //   KSPLIT = true : item = (modulus, K half, tile pair).  The pair that owns tile pair t2 of modulus mi runs BOTH halves (first
 //                   the lower half of all its tiles of the modulus, then the upper half), so the thread that stored a residue byte
 //                   of the lower half is the one that adds the upper half to it -- no cross-CTA ordering is needed.  The CTA pairs
-//                   in flight then share panels of K / 2 residue bytes: half the L2 footprint of the unsplit order (at K = 16384,
-//                   72 MiB -> 36 MiB for 74 pairs), which is what decides whether the panels survive in L2 once the pairs have
-//                   drifted apart in k.  The leftover tile pairs of a sweep (npairs % ncl) rotate over the CTA pairs from one
-//                   modulus to the next, so the load stays balanced over the launch.
+//                   in flight then share panels of K / 2 residue bytes: half the L2 footprint of the unsplit order, which is what
+//                   decides whether the panels survive in L2 once the pairs have drifted apart in k.  The leftover tile pairs of
+//                   a sweep (npairs % ncl) rotate over the CTA pairs from one modulus to the next, so the load stays balanced
+//                   over the launch.
 template <bool KSPLIT>
 struct Oz2Items {
   int npairs, ncl, cl, nmod, nk, rot, w, cur_mi, cur_kh, cur_t2;
@@ -414,13 +400,10 @@ template <bool KSPLIT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS_P, 1) ozaki2_gemm_2sm_kernel(const OzakiGemmParams p) {
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  // barriers: full[S] (used in the leader), empty[S] (per CTA), acc_full[2] (per CTA), acc_empty[2] (used in the leader)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES2 * STAGE2_BYTES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES2 + 4);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);  // full[STAGES], empty[STAGES], per CTA
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint32_t cta_rank;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
-  const bool leader = cta_rank == 0;
   const bool gated = p.gate != nullptr && *p.gate != 0;  // uniform over the grid: both CTAs of a pair take the same path
   const int nk = p.nkc;
   const int npairs_list = p.ntiles_list >> 1;             // pairs of 128-row tiles
@@ -428,30 +411,20 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS_P, 1) o
   const int ncl = gridDim.x >> 1, cl = blockIdx.x >> 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES2; ++s) {
-      mbar_init(smem_u32(&bars[s]), 1);
-      mbar_init(smem_u32(&bars[STAGES2 + s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&bars[2 * STAGES2 + b]), 1);                  // acc_full: one multicast commit
-      mbar_init(smem_u32(&bars[2 * STAGES2 + 2 + b]), 2 * EPI_WARPS);  // acc_empty (leader): every epilogue warp of the pair
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(smem_u32(&bars[s]), 1);                            // full: own producer's arrive.expect_tx (A' + both halves of B')
+      mbar_init(smem_u32(&bars[STAGES + s]), 2 * CONSUMER_WARPS);  // empty: every consumer warp of the pair
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS_P) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ===== TMA producer: this CTA's 128 rows of A' and 128 of the tile's 256 rows of B' =====
-    if (lane == 0) {
+  if (warp < 4) {
+    producer_regs();
+    // ===== TMA producer: this CTA's 128 rows of A', and 128 of the tile's 256 rows of B' for both CTAs =====
+    if (warp == 0 && lane == 0) {
       int it = 0;
       Oz2Items<KSPLIT> items(npairs_list, ncl, cl, nmod_run, nk);
       int mi, t2, kc0, kcn;
@@ -462,124 +435,41 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS_P, 1) o
         const void* tmA = p.tmaps + static_cast<size_t>(mi) * 128;
         const void* tmB = p.tmaps + static_cast<size_t>(2 * p.nmod + mi) * 128;  // the {128, 128}-box maps of B'
         for (int kc = kc0; kc < kc0 + kcn; ++kc, ++it) {
-          const int st = it % STAGES2;
-          const uint32_t ph = (it / STAGES2) & 1;
-          mbar_wait(smem_u32(&bars[STAGES2 + st]), ph ^ 1);                  // own empty barrier
-          const uint32_t full_leader = mapa_u32(smem_u32(&bars[st]), 0);     // the pair's full barrier lives in CTA 0
-          if (leader) mbar_arrive_expect_tx(smem_u32(&bars[st]), 2 * STAGE2_BYTES);
-          asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                       ::"r"(smem_u32(smem + st * STAGE2_BYTES)), "l"(tmA), "r"(full_leader), "r"(kc * BKB), "r"(m0) : "memory");
-          asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                       ::"r"(smem_u32(smem + st * STAGE2_BYTES + A_BYTES)), "l"(tmB), "r"(full_leader), "r"(kc * BKB), "r"(n0) : "memory");
+          const int st = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          mbar_wait(smem_u32(&bars[STAGES + st]), ph ^ 1);  // released by both CTAs: the peer's copy of the stage is written too
+          const uint32_t full = smem_u32(&bars[st]);
+          mbar_arrive_expect_tx(full, STAGE_BYTES);
+          tma_2d(smem_u32(smem + st * STAGE_BYTES), tmA, kc * BKB, m0, full);
+          tma_2d_multicast(smem_u32(smem + st * STAGE_BYTES + A_BYTES) + cta_rank * B2_BYTES, tmB, kc * BKB, n0, full, 3);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: the leader's elected lane drives both tensor cores (M = 256 across the pair) =====
-    if (leader && lane == 0) {
-      const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(BN >> 3) << 17) | (static_cast<uint32_t>((2 * BM) >> 4) << 24);
-      int it = 0, lt = 0;
-      Oz2Items<KSPLIT> items(npairs_list, ncl, cl, nmod_run, nk);
-      int mi, t2, kc0, kcn;
-      bool add;
-      for (; items.next(mi, t2, kc0, kcn, add); ++lt) {
-        const int buf = lt & 1;
-        const uint32_t aph = (lt >> 1) & 1;
-        mbar_wait(smem_u32(&bars[2 * STAGES2 + 2 + buf]), aph ^ 1);  // both CTAs' epilogues have drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + static_cast<uint32_t>(buf * BN);
-        for (int kc = 0; kc < kcn; ++kc, ++it) {   // kc counts within the item: the first MMA of an item overwrites the accumulator
-          const int st = it % STAGES2;
-          const uint32_t ph = (it / STAGES2) & 1;
-          mbar_wait(smem_u32(&bars[st]), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a0 = smem_u32(smem + st * STAGE2_BYTES), b0 = a0 + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BKB / UMMA_K; ++k) {
-            const uint64_t da = umma_desc_k_sw128(a0 + k * UMMA_K), db = umma_desc_k_sw128(b0 + k * UMMA_K);
-            const uint32_t acc = (kc | k) != 0;
-            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tacc),
-                         "l"(da), "l"(db), "r"(idesc), "r"(acc)
-                         : "memory");
-          }
-          // the stage is free in BOTH CTAs once these MMAs retire
-          asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                           smem_u32(&bars[STAGES2 + st])),
-                       "h"(static_cast<uint16_t>(3))
-                       : "memory");
-        }
-        asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                         smem_u32(&bars[2 * STAGES2 + buf])),
-                     "h"(static_cast<uint16_t>(3))
-                     : "memory");
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: own 128 TMEM lanes -> residues -> compact plane of this CTA's tile =====
-    const int ew = warp - 4;
-    const int q = ew & 3;
-    const int half = ew >> 2;
-    const uint32_t acc_empty_leader = mapa_u32(smem_u32(&bars[2 * STAGES2 + 2]), 0);  // + 8 * buf
-    int lt = 0;
+  } else {
+    consumer_regs();
+    // ===== consumers: own 128 rows x the pair's 256 columns -> residues -> compact plane of this CTA's tile =====
+    const int cw = (warp - 4) >> 2, wq = warp & 3;
+    const int trow = 64 * cw + 16 * wq + (lane >> 2);
+    const uint32_t empty0 = mapa_u32(smem_u32(&bars[STAGES]), 0), empty1 = mapa_u32(smem_u32(&bars[STAGES]), 1);
+    int32_t acc[128];
+    int it = 0;
     Oz2Items<KSPLIT> items(npairs_list, ncl, cl, nmod_run, nk);
     int mi, t2, kc0, kcn;
     bool add;
-    for (; items.next(mi, t2, kc0, kcn, add); ++lt) {
+    while (items.next(mi, t2, kc0, kcn, add)) {
       const int t = 2 * t2 + static_cast<int>(cta_rank);
-      const int buf = lt & 1;
-      const uint32_t aph = (lt >> 1) & 1;
-      mbar_wait(smem_u32(&bars[2 * STAGES2 + buf]), aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tsrc = tmem_base + static_cast<uint32_t>(buf * BN) + (static_cast<uint32_t>(q * 32) << 16) + half * 128;
-      const int pm = p.mod_p[mi];
-      const double pinv = p.mod_inv[mi];
-      int8_t* dst_row = p.planes + static_cast<size_t>(mi) * p.plane_stride + static_cast<size_t>(t) * (BM * BN) +
-                        static_cast<size_t>(q * 32 + lane) * BN + half * 128;
-#pragma unroll 1
-      for (int c = 0; c < 128; c += 16) {
-        uint32_t r[16];
-        TMEM_LD16(tsrc + c, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (c == 128 - 16) {
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(acc_empty_leader + 8u * static_cast<uint32_t>(buf));
-        }
-        uint32_t prev[4] = {0u, 0u, 0u, 0u};
-        if constexpr (KSPLIT) {
-          // upper K half: the residue this SAME thread stored for the lower half joins the sum before the reduction
-          // ((x mod p) + y) mod p = (x + y) mod p; |y| <= K/2 * 2^14 and x < 256 keep the sum far inside int32
-          if (add) {
-            const uint4 pv = *reinterpret_cast<const uint4*>(dst_row + c);
-            prev[0] = pv.x;
-            prev[1] = pv.y;
-            prev[2] = pv.z;
-            prev[3] = pv.w;
-          }
-        }
-        uint32_t packed[4];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint32_t wv = 0;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            int v = static_cast<int32_t>(r[4 * g + j]);
-            if constexpr (KSPLIT) v += static_cast<int>((prev[g] >> (8 * j)) & 0xffu);
-            int res = v - __double2int_rn(static_cast<double>(v) * pinv) * pm;
-            res += (res >> 31) & pm;
-            wv |= static_cast<uint32_t>(res) << (8 * j);
-          }
-          packed[g] = wv;
-        }
-        *reinterpret_cast<uint4*>(dst_row + c) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-      }
+      consume_item(acc, smem, bars, cw * 64 * BKB, kcn, it, lane, [&](int st) {
+        mbar_arrive_cluster(empty0 + 8u * static_cast<uint32_t>(st));
+        mbar_arrive_cluster(empty1 + 8u * static_cast<uint32_t>(st));
+      });
+      int8_t* tile = p.planes + static_cast<size_t>(mi) * p.plane_stride + static_cast<size_t>(t) * (BM * BN);
+      if (KSPLIT && add) store_residues<true>(acc, tile, trow, lane, p.mod_p[mi], p.mod_inv[mi]);
+      else store_residues<false>(acc, tile, trow, lane, p.mod_p[mi], p.mod_inv[mi]);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");  // nobody leaves while the peer may still signal / read
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");  // nobody leaves while the peer may still signal / write
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-  if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS_P) : "memory");
 }
 
 // ---- pass 1: per-row / per-column maximum magnitude (as the IEEE bit pattern, which orders like the value) -------
@@ -1057,7 +947,7 @@ __global__ void __launch_bounds__(256) oz2_fixup_kernel(const Oz2FixOut* __restr
 }
 
 // ---- fp32 path (BASELINE configs[3]): 3xTF32 split.  hi = tf32(a), lo = tf32(a - hi); A B ~= hi hi' + hi lo' + lo hi'
-// with fp32 accumulation in TMEM.  out_hi/out_lo[line * Kpad + k] (fp32, K contiguous), same staging as slice_kernel.
+// with fp32 accumulation in the tensor core.  out_hi/out_lo[line * Kpad + k] (fp32, K contiguous), same staging as slice_kernel.
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
@@ -1208,10 +1098,15 @@ cudaError_t for_block_chunks(int nblocks, Launch&& launch) {
   return cudaSuccess;
 }
 
-cudaError_t configure_gemm_kernel(size_t smem_bytes) {
+cudaError_t configure_gemm_kernels() {
   static PerDeviceOnce once;
   return once.run([&] {
-    return cudaFuncSetAttribute(ozaki_gemm_i8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_bytes));
+    const int bytes = static_cast<int>(GEMM_SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(ozaki_gemm_i8_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ozaki_gemm_i8_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ozaki2_gemm_2sm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ozaki2_gemm_2sm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    return e;
   });
 }
 
@@ -1234,8 +1129,7 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
   if (M <= 0 || N <= 0 || K <= 0) return cudaSuccess;
   const int S = slices < 2 ? 2 : (slices > 7 ? 7 : slices);
   const int64_t Mpad = (M + BM - 1) / BM * BM, Npad = (N + BN - 1) / BN * BN, Kpad = (K + BKB - 1) / BKB * BKB;
-  const size_t smem_bytes = 1024 + STAGES * STAGE_BYTES + (2 * STAGES + 4) * 8 + 16;
-  OZ_CHECK(configure_gemm_kernel(smem_bytes));
+  OZ_CHECK(configure_gemm_kernels());
   // block descriptor tables
   std::vector<OzBlock> ha(na), hb(nb);
   int max_ar = 1, max_ac = 1, max_br = 1, max_bc = 1;
@@ -1328,14 +1222,11 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
   p.nbc = nbc;
   p.S = S;
   p.kstep = BKB;
-  p.f32_acc = 0;
   p.kc0 = 0;
   p.nkc = static_cast<int32_t>(Kpad / BKB);
-  // D = S32 (2 @ bit 4); A, B = signed 8-bit (1 @ bits 7 and 10); both K-major; N >> 3 @ 17; M >> 4 @ 24
-  p.idesc = (2u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(BN >> 3) << 17) | (static_cast<uint32_t>(BM >> 4) << 24);
   p.tiles_m = static_cast<int32_t>(Mpad / BM);
   p.tiles_n = static_cast<int32_t>(Npad / BN);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t ntiles = static_cast<int64_t>(p.tiles_m) * p.tiles_n;
@@ -1352,7 +1243,7 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
       ++p.npairs;
     }
     first = false;
-    ozaki_gemm_i8_kernel<<<grid, GEMM_THREADS_P, smem_bytes, stream>>>(p);
+    ozaki_gemm_i8_kernel<false><<<grid, GEMM_THREADS_P, GEMM_SMEM_BYTES, stream>>>(p);
     OZ_CHECK(cudaGetLastError());
     *launches += 1;
   }
@@ -1419,7 +1310,7 @@ cudaError_t crt_constants(int* log2P, bool upload = true) {
 // The scaled-integer residue matrices A' mod p_t [T][Mpad][Kpad] and B' mod p_t [T][Npad][Kpad] live in slot-organised buffers:
 // slot s of A' holds one block row of A (rows [s * sstride, s * sstride + rows)), slot s of B' one block column of B.  A block
 // row / column is PREPARED (absmax -> exponents -> residues) as soon as all of its blocks have landed, independently of the
-// others, and a JOB multiplies any set of output blocks whose row and column slots are prepared: one persistent tcgen05 launch
+// others, and a JOB multiplies any set of output blocks whose row and column slots are prepared: one persistent wgmma launch
 // over (modulus x tile list) work items writing compact residue planes, then the CRT kernel over the same tile list.  That is
 // what lets the multiply run chunk by chunk behind the host->device ingest, and what panels the scratch for operands whose
 // residues do not fit the budget.  Nothing here synchronises with the host: non-finite input (and, in auto mode, a dynamic range
@@ -1430,9 +1321,9 @@ struct Oz2Engine {
   int T = 0, alpha = 0, crt_chunks = 4, blk = 0, sstride = 0, cap_r = 0, cap_c = 0, max_tiles = 0, range_bits = 0;
   int ksplit = 0;  // CTA-pair kernel walks (modulus, K half, tile pair) items (half the L2 footprint of the panels in flight): 1 = for
                    // long tile lists and deep K only, 2 = whenever K has an even number of chunks (tests)
-  bool paired = false;   // tile lists hold vertically adjacent 128-row tiles in pairs: the cta_group::2 kernel runs them
+  bool paired = false;   // tile lists hold vertically adjacent 128-row tiles in pairs: the CTA-pair kernel runs them
   int64_t K = 0, Kpad = 0, Mpad = 0, Npad = 0;
-  size_t a_stride = 0, b_stride = 0, plane_stride = 0, smem_bytes = 0;
+  size_t a_stride = 0, b_stride = 0, plane_stride = 0;
   int8_t *As = nullptr, *Bs = nullptr, *planes = nullptr;
   unsigned long long* maxb = nullptr;
   int32_t *exps = nullptr, *dims = nullptr;   // exps: [Mpad + Npad]; dims: rows per row slot [cap_r] then columns per column slot [cap_c]
@@ -1441,7 +1332,7 @@ struct Oz2Engine {
   int* rec_cnt = nullptr;                     // [cap_r + cap_c]
   const unsigned char* d_maps = nullptr;      // uploaded by the caller (oz2_host_maps)
   std::vector<unsigned char> h_maps;
-  int sms = 148;
+  int sms = 132;
   int launches = 0;
 };
 
@@ -1509,16 +1400,7 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
   e->a_stride = static_cast<size_t>(e->Mpad) * e->Kpad;
   e->b_stride = static_cast<size_t>(e->Npad) * e->Kpad;
   e->plane_stride = static_cast<size_t>(max_tiles) * (BM * BN);
-  e->smem_bytes = 1024 + STAGES * STAGE_BYTES + (2 * STAGES + 4) * 8 + 16;
-  OZ_CHECK(configure_gemm_kernel(e->smem_bytes));
-  {
-    static PerDeviceOnce once2;
-    OZ_CHECK(once2.run([&] {
-      cudaError_t e1 = cudaFuncSetAttribute(ozaki2_gemm_2sm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SMEM2_BYTES));
-      if (e1 != cudaSuccess) return e1;
-      return cudaFuncSetAttribute(ozaki2_gemm_2sm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SMEM2_BYTES));
-    }));
-  }
+  OZ_CHECK(configure_gemm_kernels());
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&e->sms, cudaDevAttrMultiProcessorCount, dev);
@@ -1635,7 +1517,7 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
 // One job: C blocks (+)= A' B' over the tiles of d_tiles (buffer tile coordinates (tm, tn), device array; the order is the
 // execution order, so the caller bands it for L2 reuse), written through d_ctab[rslot * cap_c + cslot] (nullptr = not part of
 // this job).  Lists longer than the plane capacity are processed in consecutive pieces.  ms_gemm (optional) accumulates the
-// tcgen05 launch time (events, synchronises): used for the roofline figure only.
+// residue GEMM launch time (events, synchronises): used for the roofline figure only.
 void oz2_set_ksplit(Oz2Engine* e, int level) { e->ksplit = level; }
 void oz2_set_paired(Oz2Engine* e, bool paired) { e->paired = paired && (e->max_tiles % 2 == 0) && (e->Mpad % (2 * BM) == 0); }
 bool oz2_paired(const Oz2Engine* e) { return e->paired; }
@@ -1652,7 +1534,6 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
   p.kc0 = 0;
   p.nkc = static_cast<int32_t>(e->Kpad / BKB);
   p.npairs = 1;
-  p.idesc = (2u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(BN >> 3) << 17) | (static_cast<uint32_t>(BM >> 4) << 24);
   p.tiles_m = static_cast<int32_t>(e->Mpad / BM);
   p.tiles_n = static_cast<int32_t>(e->Npad / BN);
   p.nmod = e->T;
@@ -1669,15 +1550,15 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
     p.ntiles_list = cnt;
     const int64_t nitems = static_cast<int64_t>(cnt) * e->T;
     if (ms_gemm) OZ_CHECK(cudaEventRecord(ev0, stream));
-    if (e->paired) {  // cta_group::2: one cluster of two CTAs per (modulus, tile pair) work item
+    if (e->paired) {  // one cluster of two CTAs per (modulus, tile pair) work item
       const int64_t npair_items = nitems / 2;
       const unsigned clusters = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(npair_items, e->sms / 2)));
       // K-split order (opt-in, oz2_set_ksplit): only for lists long enough that every CTA pair sweeps several tiles per (modulus, half)
       const bool ks = (p.nkc % 2 == 0) && (e->ksplit >= 2 || (e->ksplit == 1 && p.nkc >= 64 && (cnt / 2) >= 4 * static_cast<int>(clusters)));
-      if (ks) ozaki2_gemm_2sm_kernel<true><<<2 * clusters, GEMM_THREADS_P, SMEM2_BYTES, stream>>>(p);
-      else ozaki2_gemm_2sm_kernel<false><<<2 * clusters, GEMM_THREADS_P, SMEM2_BYTES, stream>>>(p);
+      if (ks) ozaki2_gemm_2sm_kernel<true><<<2 * clusters, GEMM_THREADS_P, GEMM_SMEM_BYTES, stream>>>(p);
+      else ozaki2_gemm_2sm_kernel<false><<<2 * clusters, GEMM_THREADS_P, GEMM_SMEM_BYTES, stream>>>(p);
     } else {
-      ozaki_gemm_i8_kernel<<<static_cast<unsigned>(std::min<int64_t>(nitems, e->sms)), GEMM_THREADS_P, e->smem_bytes, stream>>>(p);
+      ozaki_gemm_i8_kernel<false><<<static_cast<unsigned>(std::min<int64_t>(nitems, e->sms)), GEMM_THREADS_P, GEMM_SMEM_BYTES, stream>>>(p);
     }
     OZ_CHECK(cudaGetLastError());
     if (ms_gemm) {
@@ -1707,14 +1588,13 @@ cudaError_t oz2_fixup(Oz2Engine* e, const Oz2FixOut* d_outs, int nouts, const Oz
   return cudaSuccess;
 }
 
-// fp32 multiply on tcgen05 kind::tf32 with the 3xTF32 split (gemm_algo = 3).  Inputs are rounded to fp32, products are
-// accumulated in fp32 in TMEM, the result is stored into the fp64 output blocks.
+// fp32 multiply on wgmma tf32 with the 3xTF32 split (gemm_algo = 3).  Inputs are rounded to fp32, products are
+// accumulated in fp32 by the tensor cores, the result is stored into the fp64 output blocks.
 cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K, int64_t N,
                         double* const* h_ctab, int blk, int nbr, int nbc, int* launches, cudaStream_t stream) {
   if (M <= 0 || N <= 0 || K <= 0) return cudaSuccess;
   const int64_t Mpad = (M + BM - 1) / BM * BM, Npad = (N + BN - 1) / BN * BN, Kpad = (K + 31) / 32 * 32;
-  const size_t smem_bytes = 1024 + STAGES * STAGE_BYTES + (2 * STAGES + 4) * 8 + 16;
-  OZ_CHECK(configure_gemm_kernel(smem_bytes));
+  OZ_CHECK(configure_gemm_kernels());
   std::vector<OzBlock> ha(na), hb(nb);
   int max_ar = 1, max_ac = 1, max_br = 1, max_bc = 1;
   for (int i = 0; i < na; ++i) {
@@ -1800,7 +1680,6 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
   p.nbr = nbr;
   p.nbc = nbc;
   p.kstep = 32;
-  p.f32_acc = 1;
   p.accumulate = 0;
   p.diag_scale = 1.0;
   p.row_scale = row_corr;   // fp32 path: additive mean corrections, applied with the first K chunk
@@ -1810,11 +1689,9 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
   p.pair_a[0] = 1; p.pair_b[0] = 2;
   p.pair_a[1] = 0; p.pair_b[1] = 3;
   p.pair_a[2] = 0; p.pair_b[2] = 2;
-  // D = F32 (1 @ bit 4); A, B = TF32 (2 @ bits 7 and 10); both K-major; N >> 3 @ 17; M >> 4 @ 24
-  p.idesc = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(BN >> 3) << 17) | (static_cast<uint32_t>(BM >> 4) << 24);
   p.tiles_m = static_cast<int32_t>(Mpad / BM);
   p.tiles_n = static_cast<int32_t>(Npad / BN);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t ntiles = static_cast<int64_t>(p.tiles_m) * p.tiles_n;
@@ -1827,7 +1704,7 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
     p.kc0 = kc;
     p.nkc = std::min(chunk, stages_total - kc);
     p.accumulate = kc == 0 ? 0 : 1;
-    ozaki_gemm_i8_kernel<<<static_cast<unsigned>(std::min<int64_t>(ntiles, sms)), GEMM_THREADS_P, smem_bytes, stream>>>(p);
+    ozaki_gemm_i8_kernel<true><<<static_cast<unsigned>(std::min<int64_t>(ntiles, sms)), GEMM_THREADS_P, GEMM_SMEM_BYTES, stream>>>(p);
     OZ_CHECK(cudaGetLastError());
     *launches += 1;
   }

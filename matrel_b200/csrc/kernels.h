@@ -1,4 +1,4 @@
-// Internal interface between the C-ABI host layer (abi_*.cpp, host.h) and the sm_100a kernels.
+// Internal interface between the C-ABI host layer (abi_*.cpp, host.h) and the sm_90a kernels.
 // Not part of the public ABI (see include/matrel.h).
 #pragma once
 #include <cuda_runtime.h>
@@ -70,7 +70,7 @@ bool encode_kcontig_tmap(void* out128, const double* base, int64_t kdim, int64_t
 cudaError_t launch_gemm_f64(const GemmOut* d_outs, const GemmPair* d_pairs, const GemmTile* d_tiles,
                             int ntiles, const void* d_tmaps, int variant, cudaStream_t stream, const int* run_if = nullptr);
 
-// ---- fp64 block GEMM on tcgen05 (kind::i8) through Ozaki splitting (gemm_ozaki.cu) --------------------------------
+// ---- fp64 block GEMM on wgmma (s8) through Ozaki splitting (gemm_ozaki.cu) --------------------------------
 struct OzakiOperand {
   const double* v;     // dense block values (column-major, row-major if isT)
   int32_t rows, cols;  // logical block dims
@@ -118,7 +118,7 @@ int oz2_alpha(const Oz2Engine* e);
 int oz2_moduli(const Oz2Engine* e);
 int oz2_moduli_for(int64_t K, int requested);  // requested <= 0: chosen from K (see gemm_ozaki.cu)
 int oz2_slot_stride(const Oz2Engine* e);
-void oz2_set_paired(Oz2Engine* e, bool paired);                  // tile lists come as (2a, b), (2a + 1, b) pairs: use the 2-SM kernel
+void oz2_set_paired(Oz2Engine* e, bool paired);                  // tile lists come as (2a, b), (2a + 1, b) pairs: use the CTA-pair kernel
 bool oz2_paired(const Oz2Engine* e);
 void oz2_set_ksplit(Oz2Engine* e, int level);                    // CTA-pair kernel: (modulus, K half, tile pair) work items (see Oz2Items); 1 = large jobs, 2 = always
 int oz2_launches(Oz2Engine* e);                                  // kernels launched since the last call
@@ -127,7 +127,7 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
 cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* const* d_ctab, cudaStream_t stream, double* ms_gemm,
                          cudaEvent_t ev0, cudaEvent_t ev1);
 constexpr int kOz2TileM = 128, kOz2TileN = 256;
-// fp32 multiply on tcgen05 kind::tf32 (3xTF32 split, fp32 TMEM accumulation); same operand / output conventions.
+// fp32 multiply on wgmma tf32 (3xTF32 split, fp32 accumulation); same operand / output conventions.
 cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K, int64_t N,
                         double* const* h_ctab, int blk, int nbr, int nbc, int* launches, cudaStream_t stream);
 

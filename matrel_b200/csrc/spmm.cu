@@ -1,4 +1,4 @@
-// CSR-block x dense-block products for sm_100a: C(i,j) (+)= sum_k A(i,k) B(k,j) with A(i,k) sparse (CSR) and B(k,j) dense.
+// CSR-block x dense-block products for sm_90a: C(i,j) (+)= sum_k A(i,k) B(k,j) with A(i,k) sparse (CSR) and B(k,j) dense.
 //
 // Replaces BLAS.gemmsdd's CSR loop nests (M/matrix/BLAS.scala:375-413) and the reduceByKey(LocalMatrix.add) over k
 // (M/execution/MatfastExecutionHelper.scala:255): one launch per multiply, the K loop over the block pairs of an output block is

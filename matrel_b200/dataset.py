@@ -4,11 +4,11 @@
 and ``Dataset`` keeps the method names and argument order of M/Dataset.scala:57-152
 (``matrixMultiply``, ``transpose``/``t``, ``addElement``, ``multiplyElement``, ``divideElement``,
 ``addScalar``, ``multiplyScalar``, ``power``, ``matrixRankOneUpdate``), each forwarding to the C ABI
-(include/matrel.h) which launches the sm_100a kernels.  Execution is eager and asynchronous on the
+(include/matrel.h) which launches the sm_90a kernels.  Execution is eager and asynchronous on the
 session's CUDA stream instead of lazy through Catalyst; results are observationally the same
 because operators are pure.
 
-M/ = /root/reference/src/main/scala/org/apache/spark/sql/matfast/
+M/ = <reference>/src/main/scala/org/apache/spark/sql/matfast/
 """
 from __future__ import annotations
 

@@ -1,10 +1,10 @@
 """Grid-partitioned block multiply across the GPUs of one box: one process per GPU,
 ``torch.distributed`` for the plumbing (rendezvous, barriers, IPC handle exchange, small reductions), the
 engine's own C ABI for the data path: every rank PULLS the operand blocks it needs straight out of its
-peers' device slabs over NVLink 5 / NVSwitch with the copy engines (CUDA IPC mappings, ``mr_grid_multiply``),
-block row by block row, while its own sm_100a kernels already multiply what has arrived.
+peers' device slabs over NVLink / NVSwitch with the copy engines (CUDA IPC mappings, ``mr_grid_multiply``),
+block row by block row, while its own sm_90a kernels already multiply what has arrived.
 
-What it replaces in the reference (M/ = /root/reference/src/main/scala/org/apache/spark/sql/matfast/):
+What it replaces in the reference (M/ = <reference>/src/main/scala/org/apache/spark/sql/matfast/):
   * the 2 x groupByKey + join that co-locate A(:, k) with B(k, :) (M/execution/MatfastExecutionHelper.scala:236-249)
     -> chunked peer pulls of A along the grid row and of B along the grid column, overlapped with the multiply
     (``sharded_multiply``; the NCCL all-gather form is kept as ``sharded_multiply_allgather``);
@@ -238,7 +238,7 @@ def stream_barrier(device):
 
 
 def sharded_multiply_allgather(session, groups: GridGroups, A: ShardedMatrix, B: ShardedMatrix, planA: GridPlan, planB: GridPlan):
-    """C = A * B, C-stationary on the process grid, with NCCL all-gathers of the operand slabs (the form round 1 benchmarked;
+    """C = A * B, C-stationary on the process grid, with NCCL all-gathers of the operand slabs (the first form benchmarked;
     kept for comparison and for ranks that cannot map their peers' memory).  Returns (local C Dataset, keep-alive tensors).
 
     planA describes A (n x k), planB describes B (k x m); both share blk and the grid."""
@@ -589,10 +589,10 @@ def bench_main(args, METRIC, UNIT, fp64_peak_tflops, ClockSampler, cpu_reference
         dpeak, dpeak_src = fp64_peak_tflops()
         if on_tc:
             kern_ms = allmax(st2["tc_gemm_ms_total"] / 3.0)
-            ipeak, ipeak_src = int8_peak_tops() if int8_peak_tops else (2.0 * 1364.4, "2 x bf16 sustained")
+            ipeak, ipeak_src = int8_peak_tops() if int8_peak_tops else (1979.0, "H100 SXM data sheet, dense INT8")
             ach = st2["tc_int8_ops"] / (kern_ms * 1e-3) / 1e12
             roofline = {"bound": "tensor", "achieved": ach, "peak": ipeak, "unit": "TFLOP/s", "frac": ach / ipeak, "traffic": None,
-                        "op": "int8 multiply-add x 2 (TOPS) on tcgen05.mma kind::i8, per rank",
+                        "op": "int8 multiply-add x 2 (TOPS) on wgmma s8, per rank",
                         "kernel": "ozaki2_gemm_2sm_kernel", "kernel_ms": kern_ms,
                         "algorithmic": f"{st2['tc_int8_ops']:.4g} int8 ops per rank per step ({st2['tc_moduli']} moduli x 2 M_loc N_loc K; max-over-ranks kernel time)",
                         "peak_source": ipeak_src,
@@ -705,7 +705,7 @@ def bench_main(args, METRIC, UNIT, fp64_peak_tflops, ClockSampler, cpu_reference
             e2e_step()
         torch.cuda.synchronize()
         dist.barrier()
-        # the PCIe floor of the step on this box: the same uploads alone (all ranks at once), nothing else running
+        # the PCIe floor of the step on this host: the same uploads alone (all ranks at once), nothing else running
         t0 = time.perf_counter()
         for _ in range(2):
             eA.sharded.put_blocks(pA)
@@ -737,17 +737,17 @@ def bench_main(args, METRIC, UNIT, fp64_peak_tflops, ClockSampler, cpu_reference
             "metric": METRIC, "value": flops / (ms_max * 1e-3) / 1e9, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_max, "higher_is_better": True, "scaling": "strong",
             "vs_baseline": None, "dtype": "f64", "data": "synthetic",
-            "config": {"workload": f"{n}x{n} fp64 dense multiply, {blk}-block, grid-partitioned {plan.pr}x{plan.pc} over {world}xB200",
+            "config": {"workload": f"{n}x{n} fp64 dense multiply, {blk}-block, grid-partitioned {plan.pr}x{plan.pc} over {world}xH100",
                        "parallelism": (f"C-stationary {plan.pr}x{plan.pc} block-cyclic grid; every rank pulls A along its grid row and B along its grid "
                                        "column out of its peers' slabs (CUDA IPC, copy engines over NVLink), chunked and overlapped with the multiply; no reduction"),
                        "inputs": "U(0,1) java.util.Random streams, every block present, column-major",
-                       "l2": "per-rank operands after the pulls >> 126 MB L2; no flush needed",
-                       "gemm_algo": "auto -> Ozaki-II on tcgen05 on every rank" if on_tc else "dmma_fp64",
+                       "l2": "per-rank operands after the pulls >> 50 MB L2; no flush needed",
+                       "gemm_algo": "auto -> Ozaki-II on wgmma on every rank" if on_tc else "dmma_fp64",
                        "p2p_bytes_per_step": p2p},
             "e2e": {"value": flops / (e2e_ms * 1e-3) / 1e9, "unit": UNIT, "h2d_bytes_per_step": h2d_total,
                     "d2h_bytes_per_step": d2h_total, "ms_per_step": e2e_ms, "steps": e2e_steps,
                     "ingest_only_ms": ingest_only_ms, "pieces": nch,
-                    "note": "ingest_only_ms = the step's host->device copies alone on this box (max over ranks): the PCIe floor of the step"},
+                    "note": "ingest_only_ms = the step's host->device copies alone on this host (max over ranks): the PCIe floor of the step"},
             "gpu_launches": int(launches), "gpu_launches_per_step_per_rank": st["kernel_launches"] / args.steps,
             "roofline": roofline,
             "clocks": clocks,

@@ -1,5 +1,5 @@
 """Host-side block types mirroring the reference data model
-(/root/reference/src/main/scala/org/apache/spark/sql/matfast/matrix/MLMatrix.scala):
+(<reference>/src/main/scala/org/apache/spark/sql/matfast/matrix/MLMatrix.scala):
 ``DenseMatrix`` (:234-241), ``SparseMatrix`` (:525-543), ``MatrixBlock`` (:1205).
 
 These are plain containers for moving blocks across the C ABI (the 7-field struct of

@@ -1,6 +1,6 @@
 """Block -> partition maps, bit-exact with M/partitioner/*.scala, evaluated by the C ABI.
 
-M/ = /root/reference/src/main/scala/org/apache/spark/sql/matfast/
+M/ = <reference>/src/main/scala/org/apache/spark/sql/matfast/
 """
 from __future__ import annotations
 

@@ -6,9 +6,9 @@ pushing aggregates through their children on the way -- e.g. ``trace(A B) -> sum
 ``sum(A B) -> colSum(A) . rowSum(B)`` (:220-225), ``rowSum(A B) -> A . rowSum(B)`` (:181-185) -- which
 turns O(N^3) queries into O(N^2) ones.  This module restates that strategy: ``LazyDataset`` records
 nodes, ``execute()`` walks them with the same case analysis and runs the chosen physical operators
-eagerly through ``matrel_b200.dataset.Dataset`` (i.e. the sm_100a kernels).
+eagerly through ``matrel_b200.dataset.Dataset`` (i.e. the sm_90a kernels).
 
-M/ = /root/reference/src/main/scala/org/apache/spark/sql/matfast/
+M/ = <reference>/src/main/scala/org/apache/spark/sql/matfast/
 """
 from __future__ import annotations
 

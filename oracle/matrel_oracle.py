@@ -14,7 +14,7 @@ matrix/LocalMatrix.scala:1096-1135; see tests/golden/) and (ii) an independent d
 netlib-java 1.1.2) -- standard BLAS semantics, restated here with ``numpy.matmul``.
 
 All ``M/...`` citations are into
-/root/reference/src/main/scala/org/apache/spark/sql/matfast/.
+<reference>/src/main/scala/org/apache/spark/sql/matfast/.
 """
 from __future__ import annotations
 
@@ -693,7 +693,7 @@ def rank_one_update(left: BlockDict, lr, lc, right: BlockDict, rr, rc, blkSize,
 # (M/execution/MatfastExecution.scala:239-463).  literal=True restates the reference's index arithmetic
 # as written (it is only correct for square dense blocks: non-square transposed blocks are mis-strided,
 # CSR blocks are summed along the wrong axis, sparse ColumnSum has defect B5); literal=False is the
-# mathematically intended reduction, which is what the B200 engine computes.
+# mathematically intended reduction, which is what the GPU engine computes.
 # ----------------------------------------------------------------------------------------------
 
 

@@ -3,7 +3,7 @@
  * only tests/ and bench.py's cpu_baseline leg may load this; PARITY UNPINNED, see matrel_oracle.py).
  *
  * Restates, for all-dense column-major blocks:
- *   matrixMultiplyGeneral   /root/reference/src/main/scala/org/apache/spark/sql/matfast/execution/MatfastExecutionHelper.scala:235-263
+ *   matrixMultiplyGeneral   <reference>/src/main/scala/org/apache/spark/sql/matfast/execution/MatfastExecutionHelper.scala:235-263
  *   MLMatrix.multiply       .../matrix/MLMatrix.scala:100-104   (fresh zeroed C, gemm(1.0, A, B, 0.0, C))
  *   BLAS.gemmddd -> dgemm   .../matrix/BLAS.scala:327-346
  *   LocalMatrix.addDense    .../matrix/LocalMatrix.scala:56-63  (two toArray copies + a third array)

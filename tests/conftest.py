@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def _cuda_usable() -> bool:
@@ -21,11 +21,11 @@ def _cuda_usable() -> bool:
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu`-marked tests need a B200: on a box without a usable CUDA device they are skipped (not failed), so a plain
+    """`gpu`-marked tests need an H100: on a machine without a usable CUDA device they are skipped (not failed), so a plain
     `pytest` is green on CPU and `-m gpu` is the explicit device run."""
     if _cuda_usable():
         return
-    skip = pytest.mark.skip(reason="no usable CUDA device (gpu-marked tests run on the B200 box)")
+    skip = pytest.mark.skip(reason="no usable CUDA device (gpu-marked tests run on an H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

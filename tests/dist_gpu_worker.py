@@ -138,7 +138,7 @@ def main():
             err = float(np.max(np.abs(g.values - w.values)) / np.max(np.abs(w.values)))
             assert err <= (1e-5 if algo == 3 else 1e-12), (key, err)      # algo 3 = fp32 results (3xTF32)
         if algo == 2:
-            assert s_launches >= 8, s_launches     # absmax/slice passes + one GEMM per diagonal: the tcgen05 path really ran
+            assert s_launches >= 8, s_launches     # absmax/slice passes + one GEMM per diagonal: the tensor-core path really ran
         if algo == 4:
             assert s_launches >= 7, s_launches     # absmax x2, exp, residues x2, one GEMM launch over all moduli, CRT
         cnt = torch.tensor([len(got)], dtype=torch.int64, device=device)

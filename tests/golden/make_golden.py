@@ -6,7 +6,7 @@ matrix pictures in their comments.  This script writes those inputs down verbati
 expected outputs with plain dense numpy arithmetic on the full (un-blocked) matrices -- it does
 NOT import the oracle or the product, so it is an independent pin for both.
 
-Sources (paths under /root/reference/src/main/scala/org/apache/spark/sql/matfast/):
+Sources (paths under <reference>/src/main/scala/org/apache/spark/sql/matfast/):
   example/BasicMatrixOps.scala:107-144   b1..b4, s1, mat1, mat2 and their pictures
   matrix/LocalMatrix.scala:1096-1135     TestSparse: spmat1, spmat2, den1, den2, denV
   partitioner/*.scala, execution/MatfastExecutionHelper.scala:46-62   partitioner formulas

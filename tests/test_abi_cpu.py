@@ -36,7 +36,7 @@ def test_header_symbols_exported_and_bound():
 
 
 def test_library_is_not_older_than_its_sources():
-    """The in-tree .so is what travels to the GPU box: a source or header edited after the last build would ship a stale ABI."""
+    """The in-tree .so is what the package loads: a source or header edited after the last build would ship a stale ABI."""
     import glob
     import matrel_b200._native as N
     srcs = glob.glob(os.path.join(ROOT, "matrel_b200", "csrc", "*")) + [os.path.join(ROOT, "include", "matrel.h")]
@@ -52,14 +52,15 @@ def test_stats_struct_matches_the_header():
     assert [(n, {"int64_t": C.c_int64, "double": C.c_double}[t]) for t, n in fields] == list(N.mr_stats._fields_)
 
 
-def test_so_contains_blackwell_native_sass():
-    """UBLKCP = TMA bulk copy, DMMA = fp64 tensor pipe, SYNCS = mbarrier (B200_PROFILING.md table)."""
+def test_so_contains_hopper_native_sass():
+    """UBLKCP / UTMALDG = TMA bulk and tensor copies, DMMA = fp64 tensor pipe, IGMMA / HGMMA = wgmma (s8 / tf32), SYNCS = mbarrier."""
     import matrel_b200._native as N
     sass = subprocess.run(["cuobjdump", "-sass", N.LIB_PATH], capture_output=True, text=True).stdout
     if not sass:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in subprocess.run(["cuobjdump", "-lelf", N.LIB_PATH], capture_output=True, text=True).stdout
+    assert "sm_90a" in subprocess.run(["cuobjdump", "-lelf", N.LIB_PATH], capture_output=True, text=True).stdout
     assert sass.count("DMMA") >= 128 and "UBLKCP" in sass and "UTMALDG" in sass and "SYNCS" in sass
+    assert "IGMMA" in sass and "HGMMA" in sass
 
 
 def test_partitioners_bit_exact():

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 (kind::i8) Ozaki fp64 multiply (gemm_algo = 2) against the CPU oracle.
+"""GPU tests of the wgmma (s8) Ozaki fp64 multiply (gemm_algo = 2) against the CPU oracle.
 
 The path is an fp64 emulation: every slice product is an exact integer GEMM; the error comes from the
 final digit of the per-row / per-column aligned slicing.  Bars: north_star's 1e-5 relative, and a much

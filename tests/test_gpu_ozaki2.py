@@ -1,4 +1,4 @@
-"""GPU tests of the Ozaki scheme II fp64 multiply (gemm_algo = 4: int8 tcgen05 GEMMs of residue matrices + CRT).
+"""GPU tests of the Ozaki scheme II fp64 multiply (gemm_algo = 4: int8 wgmma GEMMs of residue matrices + CRT).
 
 The integer product of the scaled operands is recovered EXACTLY, so (a) integer-valued inputs give bit-exact
 results, and (b) the only error is the rounding of the operands to alpha bits relative to their row / column
@@ -146,7 +146,7 @@ def test_crt_matches_dmma_at_4096(oz2, session):
     assert worst <= 2e-14, worst      # the deviation is the DMMA kernel's own accumulated rounding (K = 4096)
 
 
-# ---------------------------------------------------------------------------------- job engine (round 2)
+# ---------------------------------------------------------------------------------- job engine
 def _pinned_blocks(ds):
     import torch
     pin = lambda m: mb.DenseMatrix(m.numRows, m.numCols, torch.from_numpy(m.values).pin_memory().numpy(), m.isTransposed)  # noqa: E731
@@ -154,7 +154,7 @@ def _pinned_blocks(ds):
 
 
 def test_crt_pipelined_behind_ingest_is_bit_identical(oz2):
-    """The tcgen05 path runs chunk by chunk behind the host->device ingest (residues of a block row / column as soon as it is
+    """The tensor-core path runs chunk by chunk behind the host->device ingest (residues of a block row / column as soon as it is
     complete, int8 GEMM + CRT of the output blocks it unlocks).  Row / column exponents do not depend on the chunking and the
     integer product is exact, so the blocks must equal the resident run's bit for bit -- whatever order the blocks arrive in."""
     n, blk = 2048, 256
@@ -214,7 +214,7 @@ def _adversarial(rng, n, tiny):
 
 
 def test_auto_selection_guards_in_row_dynamic_range():
-    """gemm_algo 0 (auto): the tcgen05 path is taken for data of ordinary range (element-wise error <= 1e-13 |A||B|) and
+    """gemm_algo 0 (auto): the tensor-core path is taken for data of ordinary range (element-wise error <= 1e-13 |A||B|) and
     refused ON THE DEVICE when a non-zero element lies too far below its row / column maximum -- the exact DMMA kernel then
     runs instead and the element-wise bound against |A||B| holds.  gemm_algo 4 (unguarded) shows why the guard exists."""
     rng = np.random.default_rng(7)
@@ -224,7 +224,7 @@ def test_auto_selection_guards_in_row_dynamic_range():
         Af, Bf = rng.uniform(-1, 1, (n, n)), rng.uniform(-1, 1, (n, n))
         s.reset_stats()
         got = full(from_dataset(to_dataset(s, blocks_of(Af, blk)).matrixMultiply(n, n, to_dataset(s, blocks_of(Bf, blk)), n, n, blk)), n, n, blk)
-        assert s.stats()["tc_gemm_launches"] == 1            # large regular product: the tcgen05 path was planned
+        assert s.stats()["tc_gemm_launches"] == 1            # large regular product: the tensor-core path was planned
         assert np.max(np.abs(got - Af @ Bf) / (np.abs(Af) @ np.abs(Bf))) <= 1e-13
         # adversarial rows: guard trips, DMMA result
         Af, Bf = _adversarial(rng, n, 2.0 ** -60)
@@ -247,7 +247,7 @@ def test_auto_selection_corrects_isolated_tiny_elements_exactly():
     """A handful of elements far below their row / column maximum (what any large random matrix contains by chance) do not send
     the multiply to the fallback: the residue pass leaves them out and their products are added exactly in fp64 afterwards.
     Here they are placed where they matter -- C(i0, j0) consists of nothing but such a product -- and every other element of
-    the result must be bit-identical to the unguarded tcgen05 run (proof that the tensor-core path was kept)."""
+    the result must be bit-identical to the unguarded tensor-core run (proof that the tensor-core path was kept)."""
     rng = np.random.default_rng(19)
     n, blk = 2048, 256
     Af, Bf = rng.uniform(1.0, 2.0, (n, n)), rng.uniform(1.0, 2.0, (n, n))

@@ -1,4 +1,4 @@
-"""GPU tests of the fp32 multiply on tcgen05 kind::tf32 (gemm_algo = 3, 3xTF32 split) -- BASELINE configs[3] shape.
+"""GPU tests of the fp32 multiply on wgmma tf32 (gemm_algo = 3, 3xTF32 split) -- BASELINE configs[3] shape.
 
 fp32 is not a reference feature (blocks are Array[Double]); parity is defined as: inputs rounded to fp32, oracle =
 fp64 product of those inputs, tolerance 1e-5 relative to max|C| (the north-star bar).  What makes it hold: the 3xTF32 split,
@@ -44,7 +44,7 @@ def test_tf32x3_multiply(n, k, m, blk, pt):
     want = O.matrix_multiply(A, n, k, B, k, m, blk)
     with mb.MatfastSession(device=0, gemm_algo=3) as s:
         got = from_dataset(to_dataset(s, A).matrixMultiply(n, k, to_dataset(s, B), k, m, blk))
-        # (two sum passes when the operands are fully covered), two slicing passes, the correction kernel, one tcgen05 launch per K chunk
+        # (two sum passes when the operands are fully covered), two slicing passes, the correction kernel, one wgmma launch per K chunk
         assert s.stats()["kernel_launches"] in (3 + -(-k // 2048), 5 + -(-k // 2048))
     assert_same_dataset(got, want, tol=TF32X3_TOL)          # ids / presence / shapes / flags exact
     full_g = O.assemble({k_: O.DenseMatrix(v.numRows, v.numCols, v.values) for k_, v in got.items()}, n, m, blk)

@@ -49,7 +49,7 @@ def test_swizzled_layout_gives_a_half_warp_16_distinct_8_byte_slots():
             assert len(slots) == 16, (s, row0)
 
 
-# ---- work-item order of the CTA-pair tcgen05 GEMM (matrel_b200/csrc/gemm_ozaki.cu, struct Oz2Items) ------------------------------
+# ---- work-item order of the CTA-pair wgmma GEMM (matrel_b200/csrc/gemm_ozaki.cu, struct Oz2Items) ------------------------------
 OZ_SRC = open(os.path.join(ROOT, "matrel_b200", "csrc", "gemm_ozaki.cu")).read()
 
 

@@ -1,6 +1,6 @@
 """A/B of the CTA-pair GEMM's work-item order on ONE box, back to back: oz2_ksplit 0 (modulus, tile pair) against 1 (modulus, K half,
 tile pair).  python tools/ab_ksplit.py [N] [BLK] [REPS] -> one JSON line with the whole-multiply wall time (context synchronised) and
-the tcgen05 GEMM launch time (events inside the library) per mode, interleaved 0 / 1 / 0 / 1 so that clock drift under the power cap
+the int8 GEMM launch time (events inside the library) per mode, interleaved 0 / 1 / 0 / 1 so that clock drift under the power cap
 hits both alike, plus a bit-identity check of one output block between the modes."""
 import json
 import os

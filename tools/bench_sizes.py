@@ -1,6 +1,6 @@
 """Sharded dense multiply at any north-star size / precision on the GPUs of one box (1 process per GPU; also runs with 1 GPU).
    [torchrun --nproc-per-node P] tools/bench_sizes.py N BLK ALGO [steps] [PRxPC]
-ALGO: 0 = auto (tcgen05 Ozaki-II, fp64-equivalent), 1 = fp64 DMMA, 3 = fp32 (tcgen05 kind::tf32, 3xTF32; BASELINE configs[3]).
+ALGO: 0 = auto (wgmma Ozaki-II, fp64-equivalent), 1 = fp64 DMMA, 3 = fp32 (wgmma tf32, 3xTF32; BASELINE configs[3]).
 Prints one JSON line on rank 0: ms (max over ranks, device-timed), TFLOP/s, fraction of the measured roof, and the error of one
 sampled output block per rank against numpy fp64 on the host (fp32-rounded inputs for ALGO 3), MAX over ranks."""
 import json, os, sys
@@ -90,24 +90,16 @@ with torch.cuda.stream(stream):
     barrier()
     s.stop()
 if rank == 0:
-    peaks = {}
-    try:
-        for line in open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles", "tc_peaks_r02.jsonl")):
-            d = json.loads(line)
-            peaks[d["bench"]] = d["value"]
-    except OSError:
-        pass
     tflops = 2.0 * n ** 3 / (ms * 1e-3) / 1e12
-    line = {"config": f"{n}x{n} {'fp32' if algo == 3 else 'fp64'} dense multiply, {blk}-block, {plan.pr}x{plan.pc} grid over {world}xB200",
-            "algo": {0: "auto: tcgen05 Ozaki-II (int8 residues + CRT), fp64-equivalent", 1: "fp64 DMMA (mma.sync m8n8k4)",
-                     3: "tcgen05 kind::tf32, 3xTF32 split, mean-centred, fp64 re-accumulation of 2048-deep K chunks"}.get(algo, str(algo)),
+    line = {"config": f"{n}x{n} {'fp32' if algo == 3 else 'fp64'} dense multiply, {blk}-block, {plan.pr}x{plan.pc} grid over {world}xH100",
+            "algo": {0: "auto: wgmma Ozaki-II (int8 residues + CRT), fp64-equivalent", 1: "fp64 DMMA (mma.sync m8n8k4)",
+                     3: "wgmma tf32, 3xTF32 split, mean-centred, fp64 re-accumulation of 2048-deep K chunks"}.get(algo, str(algo)),
             "n_gpus": world, "ms_per_step": ms, "TFLOPs": tflops, "max_rel_err_sampled_blocks": err, "tc_path": bool(st["tc_gemm_launches"])}
-    if algo == 3 and "tcgen05_tf32_sustained" in peaks:
+    if algo == 3:
         line["raw_tf32_TFLOPs"] = 3 * tflops
-        line["frac_of_measured_tf32_peak"] = 3 * tflops / (world * peaks["tcgen05_tf32_sustained"])
-        line["fp32_equiv_frac_of_peak_over_3"] = tflops / (world * peaks["tcgen05_tf32_sustained"] / 3)
+        line["frac_of_datasheet_tf32"] = 3 * tflops / (world * 495.0)    # H100 SXM data sheet, dense TF32 (not measured)
     if algo in (0, 1):
-        line["x_dmma_roof"] = tflops / (world * 37.073)
+        line["x_datasheet_fp64_tensor"] = tflops / (world * 67.0)        # H100 SXM data sheet, FP64 tensor core (not measured)
     print(json.dumps(line), flush=True)
 if world > 1:
     dist.barrier()

@@ -1,8 +1,7 @@
-// Microbenchmark: register-resident fp64 peaks on sm_100a.
+// Microbenchmark: register-resident fp64 peaks on sm_90a.
 //   (1) DMMA  : mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 chains
 //   (2) DFMA  : fma.rn.f64 chains
-// Prints JSON lines; used to fill profiles/fp64_peaks_r01.json (roofline denominator
-// for the block-GEMM kernel: SURVEY.md section 8d asks for a MEASURED DMMA peak).
+// Prints JSON lines (a measured DMMA ceiling for the block-GEMM kernel's roofline).
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
 #!/bin/bash
-# compute-sanitizer passes over the hand-written kernels (run under gpurun); summaries go to gpurun_out/.
+# compute-sanitizer passes over the hand-written kernels ; summaries go to the output directory (default sanitizer_out/).
 set -u
-OUT=${1:-gpurun_out}
+OUT=${1:-sanitizer_out}
 mkdir -p "$OUT"
 FILES="tests/test_gpu_parity.py tests/test_gpu_ozaki.py tests/test_gpu_ozaki2.py tests/test_gpu_tf32.py tests/test_gpu_spmm.py tests/test_gpu_grid.py"
 run() {  # tool, tag, pytest -k expression
