@@ -292,6 +292,11 @@ MR_JNI(jlong, dmatrixMultiply)(JNIEnv* env, jclass, jlong a, jlong b) {
   if (throw_if(env, mr_dmatrix_multiply(ptr<mr_dmatrix>(a), ptr<mr_dmatrix>(b), &out))) return 0;
   return reinterpret_cast<jlong>(out);
 }
+MR_JNI(jlong, dmatrixMultiplySplitK)(JNIEnv* env, jclass, jlong a, jlong b) {
+  mr_dmatrix* out = nullptr;
+  if (throw_if(env, mr_dmatrix_multiply_ksplit(ptr<mr_dmatrix>(a), ptr<mr_dmatrix>(b), &out))) return 0;
+  return reinterpret_cast<jlong>(out);
+}
 MR_JNI(jlong, dmatrixElementwise)(JNIEnv* env, jclass, jint op, jlong a, jlong b) {
   mr_dmatrix* out = nullptr;
   if (throw_if(env, mr_dmatrix_elementwise(op, ptr<mr_dmatrix>(a), ptr<mr_dmatrix>(b), &out))) return 0;

@@ -56,6 +56,7 @@ private[b200] object Native {
   @native def dmatrixBlockArrays(m: Long, rid: Int, cid: Int, colPtrs: Array[Int], rowIndices: Array[Int], values: Array[Double]): Unit
   @native def dmatrixOwner(m: Long, rid: Int, cid: Int): Int
   @native def dmatrixMultiply(a: Long, b: Long): Long
+  @native def dmatrixMultiplySplitK(a: Long, b: Long): Long
   @native def dmatrixElementwise(op: Int, a: Long, b: Long): Long
   @native def dmatrixReduceScalar(a: Long, what: Int): Double
   @native def dmatrixRepartition(a: Long, newPr: Int, newPc: Int): Long
@@ -183,6 +184,10 @@ class B200GridDataset private[b200](val session: B200GridSession, private[b200] 
   }
   /** Dataset.matrixMultiply (:134-142); the dimensions travel with the handles */
   def matrixMultiply(right: B200GridDataset): B200GridDataset = wrap(Native.dmatrixMultiply(h, right.h), nrows, right.ncols)
+  /** The same product split over K (matrixMultiplyGeneral's join + reduceByKey(add), MatfastExecutionHelper.scala:235-263): for
+   *  products with few output blocks (Gram matrices, low-rank factors); the partials are summed in GPU order, bit-reproducibly */
+  def matrixMultiplySplitK(right: B200GridDataset): B200GridDataset =
+    wrap(Native.dmatrixMultiplySplitK(h, right.h), nrows, right.ncols)
   def addElement(right: B200GridDataset): B200GridDataset = wrap(Native.dmatrixElementwise(0, h, right.h), nrows, ncols)
   def multiplyElement(right: B200GridDataset): B200GridDataset = wrap(Native.dmatrixElementwise(1, h, right.h), nrows, ncols)
   def divideElement(right: B200GridDataset): B200GridDataset = wrap(Native.dmatrixElementwise(2, h, right.h), nrows, ncols)

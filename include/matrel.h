@@ -306,6 +306,14 @@ MR_API mr_status mr_dmatrix_has_block(const mr_dmatrix* m, int32_t rid, int32_t 
 MR_API mr_status mr_dmatrix_num_blocks(const mr_dmatrix* m, int64_t* out);
 /* Dataset.matrixMultiply :134-142 */
 MR_API mr_status mr_dmatrix_multiply(mr_dmatrix* A, mr_dmatrix* B, mr_dmatrix** out);
+/* The same product split over K, the reference's own algorithm (matrixMultiplyGeneral, MatfastExecutionHelper.scala:235-263: join
+ * A(:, k) with B(k, :), reduceByKey(add) of the partial blocks at :255), for products whose C has fewer block rows than pr or block
+ * columns than pc (Gram matrices A^T A, factors of low rank).  With n GPUs and nbk = ceil(K / blk), GPU g multiplies the k-blocks
+ * [floor(g nbk / n), floor((g + 1) nbk / n)), pulling the blocks it lacks from their owners under the operands' own placement;
+ * every owner then sums its C blocks' partials over NVLink in ascending GPU order, starting from GPU 0's partial, so the result is
+ * bit-reproducible.  Errors as mr_dmatrix_multiply; the result is laid out exactly like its result (ids, shapes, owners, dense
+ * column-major blocks).  On a 1-GPU grid this is mr_dmatrix_multiply. */
+MR_API mr_status mr_dmatrix_multiply_ksplit(mr_dmatrix* A, mr_dmatrix* B, mr_dmatrix** out);
 /* Dataset.addElement / multiplyElement / divideElement :105-132 on co-partitioned operands (op 0 / 1 / 2): no block moves */
 MR_API mr_status mr_dmatrix_elementwise(int32_t op, mr_dmatrix* A, mr_dmatrix* B, mr_dmatrix** out);
 /* Dataset.sum / trace :73-82 (what = 0 / 1): local reduction kernels + one ncclAllReduce */

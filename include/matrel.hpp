@@ -281,6 +281,13 @@ class DistributedDataset {
     check(mr_dmatrix_multiply(h_.get(), right.h_.get(), &o));
     return DistributedDataset(*grid_, o);
   }
+  // The same product split over K (matrixMultiplyGeneral's join + reduceByKey(add)): every GPU multiplies a range of k-blocks and
+  // the owners sum the partials in GPU order; for products with few output blocks (Gram matrices, low-rank factors)
+  DistributedDataset matrixMultiplySplitK(const DistributedDataset& right) const {
+    mr_dmatrix* o = nullptr;
+    check(mr_dmatrix_multiply_ksplit(h_.get(), right.h_.get(), &o));
+    return DistributedDataset(*grid_, o);
+  }
   DistributedDataset addElement(const DistributedDataset& right) const { return elementwise(0, right); }
   DistributedDataset multiplyElement(const DistributedDataset& right) const { return elementwise(1, right); }
   DistributedDataset divideElement(const DistributedDataset& right) const { return elementwise(2, right); }

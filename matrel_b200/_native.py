@@ -169,6 +169,7 @@ SIGNATURES = {
     "mr_dmatrix_has_block": [_P, _i32, _i32, C.POINTER(_i32)],
     "mr_dmatrix_num_blocks": [_P, C.POINTER(_i64)],
     "mr_dmatrix_multiply": [_P, _P, _PP],
+    "mr_dmatrix_multiply_ksplit": [_P, _P, _PP],
     "mr_dmatrix_elementwise": [_i32, _P, _P, _PP],
     "mr_dmatrix_reduce_scalar": [_P, _i32, C.POINTER(_f64)],
     "mr_dmatrix_repartition": [_P, _i32, _i32, _PP],

@@ -617,6 +617,13 @@ mr_matrix* ensure_sharded(mr_matrix* part, const ShardLayout& L, std::unique_ptr
   return keep.get();
 }
 
+// The same, but a slab in layout L whose blocks carry the isTransposed flag (the result of a transpose) is used as it is: the
+// multiply reads row-major blocks directly.
+mr_matrix* slab_form(mr_matrix* part, const ShardLayout& L, std::unique_ptr<mr_matrix>& keep) {
+  if (part->shard && part->shard->L.same_as(L)) return part;
+  return ensure_sharded(part, L, keep);
+}
+
 
 // Moves every block of `A` into the slab of its owner in `res` (same GPUs, `res` carries its own dims and placement): block
 // (i, j) keeps its id (re-partitioning) or becomes block (j, i) (transpose; the payload is reinterpreted, not rewritten, and the
@@ -992,6 +999,204 @@ mr_status mr_dmatrix_multiply(mr_dmatrix* A_in, mr_dmatrix* B_in, mr_dmatrix** o
         if (cc != c) CUDA_CHECK(cudaStreamWaitEvent(g->ctx[i]->stream, g->ev_done[r * pc + cc], 0));
       for (int rr = 0; rr < pr; ++rr)
         if (rr != r) CUDA_CHECK(cudaStreamWaitEvent(g->ctx[i]->stream, g->ev_done[rr * pc + c], 0));
+    }
+    *out = res.release();
+  });
+}
+
+// Dataset.matrixMultiply with the reference's own algorithm (matrixMultiplyGeneral, M/execution/MatfastExecutionHelper.scala:235-263:
+// join A(:, k) with B(k, :), then reduceByKey(add) of the partial blocks at :255), for products whose C has too few blocks to
+// keep every GPU busy under mr_dmatrix_multiply (Gram matrices, factors of low rank).  With n GPUs and nbk = ceil(K / blk):
+//   1. rank g takes the k-blocks [g nbk / n, (g + 1) nbk / n) (possibly none);
+//   2. it pulls every A(i, k) / B(k, j) of its range that it does not own, from the owner under the OPERAND's placement, with the
+//      copy engines on p2p_stream, k by k (one event + ingest sequence number per k); flag-transposed slabs are pulled as they are;
+//   3. one multiply_impl over the panel (global M and N, K = the width of the range) writes its partial of EVERY C block into a
+//      partial buffer laid out the same on every rank: segment q (q * c_slots slots) is rank q's C slab, block (i, j) at its slot;
+//   4. every owner sums its blocks' windows of the contributing ranks' buffers, in rank order, straight over NVLink
+//      (ksplit_reduce_kernel) into a zeroed result slab.
+// The result is laid out exactly like mr_dmatrix_multiply's.  p2p_bytes counts the payload each rank pulled and the payload its
+// reduction read from peers.  Why not ncclReduceScatter: DESIGN.md section 5.
+mr_status mr_dmatrix_multiply_ksplit(mr_dmatrix* A, mr_dmatrix* B, mr_dmatrix** out) {
+  return guarded([&] {
+    MR_REQUIRE(A && B && out, MR_EINVAL, "null argument");
+    MR_REQUIRE(A->g == B->g, MR_EINVAL, "operands live on different grids");
+    MR_REQUIRE(A->blk == B->blk, MR_EINVAL, "operands have different block sizes (%d, %d)", A->blk, B->blk);
+    MR_REQUIRE(A->ncols == B->nrows, MR_EDIM, "Matrix dimension not match, leftColNum = %lld, rightRowNum = %lld",
+               (long long)A->ncols, (long long)B->nrows);
+    mr_grid* g = A->g;
+    const int n = g->n;
+    if (n == 1) {
+      const mr_status st = mr_dmatrix_multiply(A, B, out);
+      if (st != MR_OK) throw MrError{st, g_last_error};
+      return;
+    }
+    MR_REQUIRE(n <= kKsplitMaxParts, MR_EINVAL, "K-split multiply over %d GPUs: at most %d", n, kKsplitMaxParts);
+    const int32_t blk = A->blk;
+    const int64_t nbi = ceil_div(A->nrows, blk), nbk = ceil_div(A->ncols, blk), nbj = ceil_div(B->ncols, blk);
+    const size_t slot_elems = static_cast<size_t>(blk) * blk, slot_bytes = slot_elems * sizeof(double);
+    auto extent = [&](int64_t len, int64_t b) { return static_cast<int32_t>(std::min<int64_t>(blk, len - b * blk)); };
+    auto k_begin = [&](int rank) { return nbk * rank / n; };
+    auto res = new_dmatrix(g, A->nrows, B->ncols, blk);
+    const ShardLayout LC = layout_of(res.get(), 0);  // slot(i, j) and local_slots() are the same on every rank
+    const int64_t c_slots = LC.local_slots();
+    // operands in slab form on every rank, each under its own placement
+    std::vector<std::unique_ptr<mr_matrix>> keepA(n), keepB(n);
+    std::vector<mr_matrix*> pa(n), pb(n);
+    for (int i = 0; i < n; ++i) {
+      DeviceScope dev(g->ctx[i]);
+      std::lock_guard<std::mutex> lock(g->ctx[i]->mu);
+      pa[i] = slab_form(A->part[i], layout_of(A, i), keepA[i]);
+      pb[i] = slab_form(B->part[i], layout_of(B, i), keepB[i]);
+      CUDA_CHECK(cudaEventRecord(g->ctx[i]->ev_alloc, g->ctx[i]->h2d_stream));
+      CUDA_CHECK(cudaStreamWaitEvent(g->ctx[i]->stream, g->ctx[i]->ev_alloc, 0));
+      CUDA_CHECK(cudaEventRecord(g->ev_ready[i], g->ctx[i]->stream));  // "my slabs are complete"
+    }
+    // ---- pulls + partial products
+    std::vector<Buf> partial(n);
+    std::vector<std::unique_ptr<mr_matrix>> products(n);
+    for (int r = 0; r < n; ++r) {
+      mr_context* ctx = g->ctx[r];
+      DeviceScope dev(ctx);
+      std::lock_guard<std::mutex> lock(ctx->mu);
+      const int64_t k0 = k_begin(r), k1 = k_begin(r + 1);
+      if (k1 > k0) {
+        struct Src {
+          std::pair<int32_t, int32_t> id;
+          int owner;
+          bool left;
+        };
+        std::vector<Src> remote;
+        size_t panel_bytes = 0;
+        std::vector<char> from(n, 0);
+        for (int64_t k = k0; k < k1; ++k) {
+          for (int64_t i = 0; i < nbi; ++i) {
+            const int o = A->owner(static_cast<int32_t>(i), static_cast<int32_t>(k));
+            if (o == r) continue;
+            remote.push_back({{static_cast<int32_t>(i), static_cast<int32_t>(k)}, o, true});
+            panel_bytes += align_up(static_cast<size_t>(extent(A->nrows, i)) * extent(A->ncols, k) * sizeof(double));
+            from[o] = 1;
+          }
+          for (int64_t j = 0; j < nbj; ++j) {
+            const int o = B->owner(static_cast<int32_t>(k), static_cast<int32_t>(j));
+            if (o == r) continue;
+            remote.push_back({{static_cast<int32_t>(k), static_cast<int32_t>(j)}, o, false});
+            panel_bytes += align_up(static_cast<size_t>(extent(B->nrows, k)) * extent(B->ncols, j) * sizeof(double));
+            from[o] = 1;
+          }
+        }
+        Buf panel = std::make_shared<DevBuf>(ctx, std::max<size_t>(panel_bytes, 16));
+        partial[r] = std::make_shared<DevBuf>(ctx, static_cast<size_t>(n) * c_slots * slot_bytes);
+        cudaStream_t ps = ctx->p2p_stream;
+        CUDA_CHECK(cudaEventRecord(ctx->ev_order, ctx->stream));  // the pulls follow the panel allocation ...
+        CUDA_CHECK(cudaStreamWaitEvent(ps, ctx->ev_order, 0));
+        for (int o = 0; o < n; ++o)                                 // ... and the owners' slabs
+          if (from[o]) CUDA_CHECK(cudaStreamWaitEvent(ps, g->ev_ready[o], 0));
+        std::unique_ptr<mr_matrix> tA(new_matrix(ctx)), tB(new_matrix(ctx));
+        // a block of the panel: own blocks are windows of the own slab (keeping their producer's event), the others are pulled
+        auto place = [&](mr_dmatrix* M, const std::vector<mr_matrix*>& parts, mr_matrix* dst, std::pair<int32_t, int32_t> id,
+                         std::pair<int32_t, int32_t> key, const ReadyPtr& ready, uint64_t seq, size_t* panel_off, int64_t* pulled) {
+          const int o = M->owner(id.first, id.second);
+          const ShardInfo& sh = *parts[o]->shard;
+          const int32_t br = extent(M->nrows, id.first), bc = extent(M->ncols, id.second);
+          const size_t src_off = static_cast<size_t>(sh.L.slot(id.first, id.second)) * slot_bytes;
+          if (o == r) {
+            Block b = dense_block(br, bc, Span{sh.slab, src_off}, sh.isT);
+            auto it = parts[o]->blocks.find(id);
+            if (it != parts[o]->blocks.end()) {
+              b.ready = it->second.ready;
+              b.settled = it->second.settled;
+            }
+            b.seq = seq;
+            dst->blocks[key] = std::move(b);
+            return;
+          }
+          const size_t bytes = static_cast<size_t>(br) * bc * sizeof(double);
+          CUDA_CHECK(cudaMemcpyAsync(static_cast<char*>(panel->p) + *panel_off, static_cast<const char*>(sh.slab->p) + src_off, bytes,
+                                     cudaMemcpyDefault, ps));
+          Block b = dense_block(br, bc, Span{panel, *panel_off}, sh.isT);
+          b.ready = ready;
+          b.seq = seq;
+          dst->blocks[key] = std::move(b);
+          *panel_off += align_up(bytes);
+          *pulled += static_cast<int64_t>(bytes);
+        };
+        size_t panel_off = 0;
+        int64_t pulled = 0;
+        for (int64_t k = k0; k < k1; ++k) {  // ascending k: the multiply can start on the first k-blocks while later ones travel
+          ReadyPtr ready = std::make_shared<Ready>();
+          const uint64_t seq = ++ctx->ingest_seq;
+          const int32_t kg = static_cast<int32_t>(k), kl = static_cast<int32_t>(k - k0);
+          for (int32_t i = 0; i < nbi; ++i) place(A, pa, tA.get(), {i, kg}, {i, kl}, ready, seq, &panel_off, &pulled);
+          for (int32_t j = 0; j < nbj; ++j) place(B, pb, tB.get(), {kg, j}, {kl, j}, ready, seq, &panel_off, &pulled);
+          CUDA_CHECK(cudaEventRecord(ready->ev, ps));
+          panel->ready = ready;  // the panel is released after its last pull
+        }
+        ctx->stats.p2p_bytes += pulled;
+        Buf part = partial[r];
+        const OutWindowFn window = [&](int32_t i, int32_t j) {
+          return Span{part, static_cast<size_t>(res->owner(i, j) * c_slots + LC.slot(i, j)) * slot_bytes};
+        };
+        // the panel's k-blocks are numbered from 0 and the multiply sees K = the range's width: the Ozaki-II residue planes and the
+        // choice of engine and moduli follow the work this rank does, not the whole K
+        const int64_t k_len = std::min<int64_t>(A->ncols, k1 * blk) - k0 * blk;
+        products[r].reset(multiply_impl(ctx, tA.get(), A->nrows, k_len, tB.get(), k_len, B->ncols, blk, nullptr, &window));
+      }
+      CUDA_CHECK(cudaEventRecord(g->ev_done[r], ctx->p2p_stream));  // "my pulls are done"
+    }
+    // nobody may release / overwrite an operand slab before every peer's pulls from it have run
+    for (int i = 0; i < n; ++i) {
+      DeviceScope dev(g->ctx[i]);
+      for (int p = 0; p < n; ++p)
+        if (p != i) CUDA_CHECK(cudaStreamWaitEvent(g->ctx[i]->stream, g->ev_done[p], 0));
+    }
+    // ---- the owners' reductions, over the contributing ranks in rank order
+    std::vector<const double*> parts;
+    std::vector<int> contributors;
+    for (int r = 0; r < n; ++r)
+      if (partial[r]) {
+        parts.push_back(static_cast<const double*>(partial[r]->p));
+        contributors.push_back(r);
+        DeviceScope dev(g->ctx[r]);
+        CUDA_CHECK(cudaEventRecord(g->ev_ready[r], g->ctx[r]->stream));  // "my partial products are complete"
+      }
+    for (int q = 0; q < n; ++q) {
+      mr_context* ctx = g->ctx[q];
+      DeviceScope dev(ctx);
+      std::lock_guard<std::mutex> lock(ctx->mu);
+      res->part[q] = new_sharded(ctx, layout_of(res.get(), q), false, true);
+      std::vector<KsplitDesc> descs;
+      int64_t max_count = 0, peer_elems = 0;
+      for (auto& kv : res->part[q]->blocks) {
+        const int64_t cnt = static_cast<int64_t>(kv.second.numRows) * kv.second.numCols;
+        const int64_t offset = (static_cast<int64_t>(q) * c_slots + LC.slot(kv.first.first, kv.first.second)) * static_cast<int64_t>(slot_elems);
+        descs.push_back(KsplitDesc{kv.second.values.ptr<double>(), offset, cnt});
+        max_count = std::max(max_count, cnt);
+        peer_elems += cnt;
+      }
+      if (!descs.empty()) {
+        for (int r : contributors)
+          if (r != q) CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, g->ev_ready[r], 0));
+        Buf dd = upload(ctx, descs), dp = upload(ctx, parts);
+        CUDA_CHECK(launch_ksplit_reduce(static_cast<const KsplitDesc*>(dd->p), static_cast<int>(descs.size()),
+                                        static_cast<const double* const*>(dp->p), static_cast<int>(parts.size()), max_count, ctx->stream));
+        note_launch(ctx);
+        const int64_t peers = static_cast<int64_t>(contributors.size()) - (partial[q] ? 1 : 0);
+        ctx->stats.p2p_bytes += peer_elems * peers * static_cast<int64_t>(sizeof(double));
+      }
+      CUDA_CHECK(cudaEventRecord(g->ev_done[q], ctx->stream));  // "my reduction has read the partials"
+    }
+    // a partial buffer is released only after every owner's reduction has read it
+    for (int r : contributors) {
+      DeviceScope dev(g->ctx[r]);
+      for (int q = 0; q < n; ++q)
+        if (q != r) CUDA_CHECK(cudaStreamWaitEvent(g->ctx[r]->stream, g->ev_done[q], 0));
+      products[r].reset();
+      partial[r].reset();
+    }
+    for (int i = 0; i < n; ++i) {
+      DeviceScope dev(g->ctx[i]);
+      keepA[i].reset();
+      keepB[i].reset();
     }
     *out = res.release();
   });

@@ -611,7 +611,7 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
 }
 
 void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner& planner, int32_t blkSize,
-                  mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer) {
+                  mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows) {
   const ShardInfo* out_shard = result->shard.get();
   // Low-density sparse x sparse pairs: next to any dense partial the block sum is dense whatever the partial's own format
   // (LocalMatrix.add), so there they are ordinary sparse x dense products of the densified right operand; an output block
@@ -627,9 +627,17 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       o.spsp.clear();
     }
   }
-  // allocate all output blocks from one slab (packed in plan order, or at their slots when the result is a sharded dataset)
+  // allocate all output blocks from one slab (packed in plan order, or at their slots when the result is a sharded dataset), or
+  // take them from the caller's windows
   std::vector<double*> cptr(plans.size());
-  if (out_shard) {
+  if (out_windows) {
+    for (size_t i = 0; i < plans.size(); ++i) {
+      auto& o = plans[i];
+      Span s = (*out_windows)(o.rid, o.cid);
+      cptr[i] = s.ptr<double>();
+      result->blocks[{o.rid, o.cid}] = dense_block(o.m, o.n, s, false);
+    }
+  } else if (out_shard) {
     const ShardLayout& L = out_shard->L;
     // absent output blocks must read as zeros for whoever pulls this slab later (a sharded dataset is dense over its grid)
     if (static_cast<int64_t>(plans.size()) < L.slots_r_of(L.r) * ((L.nbc > L.c ? (L.nbc - L.c + L.pc - 1) / L.pc : 0)))
@@ -1089,7 +1097,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
 namespace mrhost {
 
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
-                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout) {
+                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows) {
   for (auto& kv : left->blocks)
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
   for (auto& kv : right->blocks)
@@ -1144,7 +1152,8 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
   }
   std::unique_ptr<mr_matrix> result(out_layout ? new_sharded(ctx, *out_layout, false, false) : new_matrix(ctx));
   if (out_layout) result->blocks.clear();  // only the blocks the product has are present (join semantics); absent ones stay absent
-  run_multiply(ctx, plans, planner, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, leftColBlkNum == 1 && rightRowBlkNum == 1);
+  run_multiply(ctx, plans, planner, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, leftColBlkNum == 1 && rightRowBlkNum == 1,
+               out_windows);
   return result.release();
 }
 

@@ -7,6 +7,7 @@
 //   sparse -> dense                  SparseMatrix.toArray (MLMatrix.scala:637-663)
 //   sparse x dense                   BLAS.gemmsdd (BLAS.scala:352-458)
 //   java.util.Random U(0,1) fill     DenseMatrix.rand (MLMatrix.scala:453-457)
+//   cross-GPU partial sum            reduceByKey(LocalMatrix.add) of matrixMultiplyGeneral (MatfastExecutionHelper.scala:255)
 // Flat paths use 128-bit ld/st.global.v2.f64 with 4 independent vectors in flight per thread;
 // layout-mixing paths stage a 32x32 tile through padded shared memory so both the row-major
 // read and the column-major write are fully coalesced.
@@ -471,6 +472,56 @@ __global__ void __launch_bounds__(256) copy_words_kernel(uint32_t* __restrict__ 
   for (size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x; i < nwords; i += static_cast<size_t>(gridDim.x) * 256) dst[i] = src[i];
 }
 
+// ---- K-split multiply: out = sum of the partial products of the contributing GPUs, in part order (kernels.h, KsplitDesc).
+// Most parts live on peer GPUs, so every load is an NVLink round trip: each thread issues the loads of a group of parts before
+// it adds any of them, and the adds then run strictly left to right (part 0's value, + part 1, + part 2, ...), which keeps the
+// result bit-reproducible.  128-bit loads and stores when every window shares the output's 16-byte phase (with an odd blk a
+// slot starts on an 8-byte boundary: one scalar element first), scalar ones otherwise.
+constexpr int KSPLIT_THREADS = 256;
+constexpr int KSPLIT_GROUP = 8;
+
+__global__ void __launch_bounds__(KSPLIT_THREADS) ksplit_reduce_kernel(const KsplitDesc* __restrict__ descs,
+                                                                      const double* const* __restrict__ parts, int nparts) {
+  __shared__ const double* src[kKsplitMaxParts];
+  const KsplitDesc d = descs[blockIdx.y];
+  for (int q = threadIdx.x; q < nparts; q += KSPLIT_THREADS) src[q] = parts[q] + d.offset;
+  __syncthreads();
+  const uintptr_t phase = reinterpret_cast<uintptr_t>(d.out) & 15;
+  bool same = true;
+  for (int q = 0; q < nparts; ++q) same = same && (reinterpret_cast<uintptr_t>(src[q]) & 15) == phase;
+  const int64_t head = same ? (phase != 0 && d.count > 0 ? 1 : 0) : d.count;  // scalar elements in front of the 128-bit body
+  const int64_t nvec = (d.count - head) >> 1;
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * KSPLIT_THREADS;
+  const int64_t t = static_cast<int64_t>(blockIdx.x) * KSPLIT_THREADS + threadIdx.x;
+  for (int64_t i = t; i < nvec; i += stride) {
+    double2 acc = make_double2(0.0, 0.0);
+    for (int q0 = 0; q0 < nparts; q0 += KSPLIT_GROUP) {
+      double2 v[KSPLIT_GROUP];
+#pragma unroll
+      for (int u = 0; u < KSPLIT_GROUP; ++u)
+        if (q0 + u < nparts) v[u] = ld_stream(reinterpret_cast<const double2*>(src[q0 + u] + head) + i);
+#pragma unroll
+      for (int u = 0; u < KSPLIT_GROUP; ++u)
+        if (q0 + u < nparts) {
+          if (q0 + u == 0) {
+            acc = v[0];
+          } else {
+            acc.x += v[u].x;
+            acc.y += v[u].y;
+          }
+        }
+    }
+    st_stream(reinterpret_cast<double2*>(d.out + head) + i, acc);
+  }
+  auto scalar = [&](int64_t e) {
+    double acc = __ldcs(src[0] + e);
+    for (int q = 1; q < nparts; ++q) acc += __ldcs(src[q] + e);
+    __stcs(d.out + e, acc);
+  };
+  for (int64_t e = t; e < head; e += stride) scalar(e);
+  for (int64_t e = head + 2 * nvec + t; e < d.count; e += stride) scalar(e);
+}
+
 inline int flat_grid_x(int64_t max_n) {
   int64_t vec = (max_n + 1) / 2;
   int64_t gx = (vec + static_cast<int64_t>(FLAT_THREADS) * FLAT_UNROLL - 1) / (static_cast<int64_t>(FLAT_THREADS) * FLAT_UNROLL);
@@ -635,6 +686,19 @@ cudaError_t launch_copy_words(void* dst, const void* src_mapped, size_t bytes, c
   size_t grid = (nwords + 255) / 256;
   if (grid > 64) grid = 64;
   copy_words_kernel<<<static_cast<unsigned>(grid), 256, 0, stream>>>(static_cast<uint32_t*>(dst), static_cast<const uint32_t*>(src_mapped), nwords);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ksplit_reduce(const KsplitDesc* d_descs, int ndescs, const double* const* d_parts, int nparts, int64_t max_count,
+                                 cudaStream_t stream) {
+  if (ndescs <= 0 || max_count <= 0) return cudaSuccess;
+  if (nparts < 1 || nparts > kKsplitMaxParts) return cudaErrorInvalidValue;
+  int64_t gx = ((max_count + 1) / 2 + KSPLIT_THREADS - 1) / KSPLIT_THREADS;  // one 128-bit element per thread
+  if (gx > 4096) gx = 4096;
+  for (int off = 0; off < ndescs; off += 65535) {  // gridDim.y limit
+    dim3 grid(static_cast<unsigned>(gx), static_cast<unsigned>(ndescs - off < 65535 ? ndescs - off : 65535));
+    ksplit_reduce_kernel<<<grid, KSPLIT_THREADS, 0, stream>>>(d_descs + off, d_parts, nparts);
+  }
   return cudaGetLastError();
 }
 

@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstring>
 #include <deque>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -240,10 +241,14 @@ struct DeviceScope {
 };
 ShardLayout make_layout(int64_t nrows, int64_t ncols, int32_t blk, int32_t pr, int32_t pc, int32_t r, int32_t c);
 mr_matrix* new_sharded(mr_context* ctx, const ShardLayout& L, bool ipc_capable, bool zero, bool isT = false);
+// Where a multiply writes output block (rid, cid): a dense column-major window the caller has allocated (at least m x n doubles).
+using OutWindowFn = std::function<Span(int32_t rid, int32_t cid)>;
 // The body of mr_matrix_multiply (abi_multiply.cpp).  out_layout != nullptr: the result is a sharded dataset in that layout
-// (its blocks are windows of one slab at their slots) instead of a packed one.  The caller holds ctx->mu.
+// (its blocks are windows of one slab at their slots) instead of a packed one.  out_windows != nullptr (with out_layout ==
+// nullptr): every output block is written into the caller's window and the result's blocks are those windows.  The caller
+// holds ctx->mu.
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
-                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout);
+                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr);
 }  // namespace mrhost
 
 namespace mrhost {

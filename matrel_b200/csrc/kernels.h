@@ -279,6 +279,20 @@ cudaError_t launch_extract_lines(const LineDesc* d_descs, int nblocks, int max_l
 // descriptor tables of an operator must not queue behind gigabytes of block ingest on the H2D engine.
 cudaError_t launch_copy_words(void* dst, const void* src_mapped, size_t bytes, cudaStream_t stream);
 
+// Cross-GPU sum of the K-split multiply's partial products (abi_grid.cpp, mr_dmatrix_multiply_ksplit):
+//   out[e] = parts[0][offset + e] + parts[1][offset + e] + ... + parts[nparts - 1][offset + e],  e < count,
+// added left to right in part order (deterministic, independent of timing).  Part pointers may be peer-device pointers: the
+// reads go over NVLink, so the roof is NVLink read bandwidth, not HBM.  `parts` is a device array of nparts (<= kKsplitMaxParts)
+// base pointers; descriptors are device memory.
+struct KsplitDesc {
+  double* out;
+  int64_t offset;  // elements, the same for every part
+  int64_t count;
+};
+constexpr int kKsplitMaxParts = 64;
+cudaError_t launch_ksplit_reduce(const KsplitDesc* d_descs, int ndescs, const double* const* d_parts, int nparts, int64_t max_count,
+                                 cudaStream_t stream);
+
 // java.util.Random-compatible U(0,1) fill: out[i] = i-th nextDouble() of new Random(seed), batched over blocks
 struct RandDesc {
   double* out;

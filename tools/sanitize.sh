@@ -4,8 +4,8 @@ set -u
 OUT=${1:-sanitizer_out}
 mkdir -p "$OUT"
 FILES="tests/test_gpu_parity.py tests/test_gpu_ozaki.py tests/test_gpu_ozaki2.py tests/test_gpu_tf32.py tests/test_gpu_spmm.py tests/test_gpu_grid.py"
-run() {  # tool, tag, pytest -k expression
-  timeout 900 compute-sanitizer --tool "$1" --print-limit 5 python -m pytest $FILES -m gpu -x -q -k "$3" > "$OUT/sanitizer_$1_$2.log" 2>&1
+run() {  # tool, tag, pytest -k expression [, test files instead of $FILES]
+  timeout 900 compute-sanitizer --tool "$1" --print-limit 5 python -m pytest ${4:-$FILES} -m gpu -x -q -k "$3" > "$OUT/sanitizer_$1_$2.log" 2>&1
   echo "== $1 $2: exit $? ; $(grep -E 'ERROR SUMMARY|RACECHECK SUMMARY|passed|failed' "$OUT/sanitizer_$1_$2.log" | tr '\n' ' ')"
 }
 run memcheck dmma    "multiply_dense_vs_oracle and (131 or 300 or 40-40)"
@@ -18,6 +18,7 @@ run memcheck spsp    "sparse_times_sparse"
 run memcheck spmm2   "spmm2_vs_oracle and (700 or 0.05 or False) or spmm2_accumulates"               # ragged strips, global-entry path, unsorted rows
 run memcheck sprand  "device_sprand and 512"
 run memcheck grid    "grid_multiply_matches_oracle and 1-4-1024 or sharded_put_block"
+run memcheck ksplit  "ksplit_matches_oracle and (1-1-gram or 2-1-odd or 2-4-k3 or 8-1-single)" tests/test_gpu_grid_ksplit.py  # world 1 and multi-GPU, 128-bit and scalar reduce paths
 run synccheck crt    "crt_multiply_vs_oracle and (256-256-256 or 1024)"
 run synccheck spmm2  "spmm2_vs_oracle and 700"
 run racecheck crt2sm "crt_multiply_vs_oracle and 1024"
