@@ -739,7 +739,10 @@ __global__ void __launch_bounds__(256) residue_kernel(const OzBlock* __restrict_
   for (int l = warp; l < 32; l += 8) {
     if (l0 + l >= nlines) continue;
     const int e = line_exp[gl_base + l];
-    const double line_scale = scalbn(1.0, alpha - e);  // exact power of two
+    // exact powers of two.  alpha - e reaches alpha + 1073 for a line of sub-normals, beyond the largest fp64 power of two: the scale
+    // is applied as two factors (the first product stays below 2^alpha, so both multiplications are exact)
+    const int sh1 = min(alpha - e, 1023);
+    const double line_scale = scalbn(1.0, sh1), line_scale2 = scalbn(1.0, alpha - e - sh1);
     uint32_t hi[4], lo[4];
     float sgn[4];
 #pragma unroll
@@ -752,7 +755,7 @@ __global__ void __launch_bounds__(256) residue_kernel(const OzBlock* __restrict_
         else *gate = 1;
         xv = 0.0;
       }
-      const long long X = __double2ll_rn(xv * line_scale);  // exact scaling, |X| <= 2^alpha
+      const long long X = __double2ll_rn(xv * line_scale * line_scale2);  // exact scaling, |X| <= 2^alpha
       sgn[j] = X < 0 ? -1.0f : 1.0f;
       const unsigned long long U = static_cast<unsigned long long>(X < 0 ? -X : X);
       hi[j] = static_cast<uint32_t>(U >> 32);

@@ -12,7 +12,8 @@ run memcheck dmma    "multiply_dense_vs_oracle and (131 or 300 or 40-40)"
 run memcheck ozaki   "ozaki_multiply_vs_oracle and (131 or 300)"
 run memcheck crt     "crt_multiply_vs_oracle and (131 or 300 or 1024) or crt_is_bit_exact"          # engine: 1-SM (blk 64/128) and CTA-pair (blk 256) kernels
 run memcheck crtjobs "crt_pipelined or crt_panelled or corrects_isolated"           # + outlier records and the fix-up kernel                                                # pipelined groups, panelled scratch
-run memcheck tf32    "tf32x3_multiply and (300 or 512)"
+run memcheck crtedge "irregular_shapes and (563x563x563-blk200-sparse or 356x300x356)" tests/test_gpu_ozaki2_edges.py   # CTA pairs on ragged slots: padding tile, absent blocks
+run memcheck tf32   "tf32x3_multiply and (300 or 512)"
 run memcheck sparse  "sparse_blocks or sparse_op_sparse or aggregates or project"
 run memcheck spsp    "sparse_times_sparse"
 run memcheck spmm2   "spmm2_vs_oracle and (700 or 0.05 or False) or spmm2_accumulates"               # ragged strips, global-entry path, unsorted rows
