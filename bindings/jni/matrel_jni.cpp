@@ -133,6 +133,28 @@ MR_JNI(jlong, matrixCreate)(JNIEnv* env, jclass, jlong ctx) {
   return reinterpret_cast<jlong>(m);
 }
 MR_JNI(void, matrixFree)(JNIEnv* env, jclass, jlong m) { throw_if(env, mr_matrix_free(ptr<mr_matrix>(m))); }
+// host-resident datasets: put_block copies the JVM arrays into page-locked memory owned by the library, so the staged
+// arrays are released as soon as the call returns
+MR_JNI(jlong, matrixCreateHost)(JNIEnv* env, jclass, jlong ctx) {
+  mr_matrix* m = nullptr;
+  if (throw_if(env, mr_matrix_create_host(ptr<mr_context>(ctx), &m))) return 0;
+  return reinterpret_cast<jlong>(m);
+}
+MR_JNI(jboolean, isHost)(JNIEnv* env, jclass, jlong m) {
+  int32_t host = 0;
+  throw_if(env, mr_matrix_is_host(ptr<mr_matrix>(m), &host));
+  return host != 0;
+}
+MR_JNI(jlong, toHost)(JNIEnv* env, jclass, jlong m) {
+  mr_matrix* out = nullptr;
+  if (throw_if(env, mr_matrix_to_host(ptr<mr_matrix>(m), &out))) return 0;
+  return reinterpret_cast<jlong>(out);
+}
+MR_JNI(jlong, toDevice)(JNIEnv* env, jclass, jlong m) {
+  mr_matrix* out = nullptr;
+  if (throw_if(env, mr_matrix_to_device(ptr<mr_matrix>(m), &out))) return 0;
+  return reinterpret_cast<jlong>(out);
+}
 MR_JNI(void, putBlock)(JNIEnv* env, jclass, jlong m, jint rid, jint cid, jbyte type, jint numRows, jint numCols, jintArray colPtrs,
                        jintArray rowIndices, jdoubleArray values, jboolean isTransposed) {
   StagedBlock b(env, type, numRows, numCols, colPtrs, rowIndices, values, isTransposed);

@@ -16,6 +16,10 @@ private[b200] object Native {
   @native def sync(ctx: Long): Unit
   @native def matrixCreate(ctx: Long): Long
   @native def matrixFree(m: Long): Unit
+  @native def matrixCreateHost(ctx: Long): Long
+  @native def isHost(m: Long): Boolean
+  @native def toHost(m: Long): Long
+  @native def toDevice(m: Long): Long
   @native def putBlock(m: Long, rid: Int, cid: Int, tpe: Byte, numRows: Int, numCols: Int,
                        colPtrs: Array[Int], rowIndices: Array[Int], values: Array[Double],
                        isTransposed: Boolean): Unit
@@ -100,6 +104,14 @@ class B200Session(device: Int = -1, compatBugs: Boolean = true, gemmAlgo: Int = 
     blocks.foreach(b => Native.put(h, b, Native.putBlock))
     new B200Dataset(this, h)
   }
+
+  /** The same, host-resident: the blocks live in page-locked host memory owned by the engine (datasets larger than the GPU);
+   *  matrixMultiply streams them through the device, every other operator needs toDevice() first */
+  def toHostDS(blocks: Seq[MatrixBlock]): B200Dataset = {
+    val h = Native.matrixCreateHost(ctx)
+    blocks.foreach(b => Native.put(h, b, Native.putBlock))
+    new B200Dataset(this, h)
+  }
 }
 
 class B200Dataset private[b200](val session: B200Session, private[b200] val h: Long) {
@@ -111,6 +123,11 @@ class B200Dataset private[b200](val session: B200Session, private[b200] val h: L
   def getBlock(rid: Int, cid: Int): MLMatrix =
     Native.readBlock(Native.blockMeta(h, rid, cid), (cp, ri, v) => Native.blockArrays(h, rid, cid, cp, ri, v))
   def collect(): Seq[MatrixBlock] = blockIds.map { case (i, j) => MatrixBlock(i, j, getBlock(i, j)) }
+
+  // ---- residence
+  def isHost: Boolean = Native.isHost(h)
+  def toHost(): B200Dataset = wrap(Native.toHost(h))
+  def toDevice(): B200Dataset = wrap(Native.toDevice(h))
 
   // ---- operators: Dataset.scala:38-152
   def project(nrows: Long, ncols: Long, blkSize: Int, rowOrCol: Boolean, index: Long): B200Dataset =

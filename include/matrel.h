@@ -85,6 +85,7 @@ MR_API mr_status mr_init(const mr_options* opts, mr_context** out);
 MR_API mr_status mr_shutdown(mr_context* ctx);
 MR_API mr_status mr_set_stream(mr_context* ctx, void* cuda_stream);
 /* keys: "compat_bugs", "gemm_algo", "ozaki_slices", "crt_moduli", "ozaki_scratch_mb", "spmm_algo", "pipeline", "time_kernels", "gemm_variant",
+ *       "stream_budget_mb" (device memory a streamed multiply may use, in MiB; 0 = free device memory at the call minus 1 GiB),
  *       "oz2_ksplit" (the CTA-pair wgmma GEMM walks (modulus, K half, tile pair) work items -- half the L2 footprint of the
  *       residue panels in flight, bit-identical results: 1 = for long tile lists and K >= 8192 only, 2 = whenever possible; default 0,
  *       or the environment variable MATREL_OZ2_KSPLIT at mr_init) */
@@ -152,6 +153,25 @@ MR_API mr_status mr_matrix_sprand(mr_context* ctx, int64_t nrows, int64_t ncols,
 MR_API mr_status mr_matrix_rand_partition(mr_context* ctx, int64_t nrows, int64_t ncols, int32_t blkSize, int64_t seed0,
                                           int32_t pr, int32_t pc, int32_t r, int32_t c, double* dslab,
                                           int64_t slotElems, mr_matrix** out);
+
+/* ---- host-resident datasets: for products larger than device memory.  The blocks live in page-locked host memory owned by
+ *      the library (allocated in chunks of up to 1 GiB, kept for reuse until mr_shutdown).  mr_matrix_put_block copies the caller's
+ *      arrays into it (they are free again when the call returns) with the same checks as a device dataset; get_block, has_block,
+ *      block_ids, num_blocks and free behave as for a device dataset.  mr_matrix_multiply streams a host-resident operand through
+ *      the device tile by tile and returns a host-resident C, bit-identical to the resident product under gemm_algo 0, 1 and 4 (DESIGN.md
+ *      section 4.6; gemm_algo 2 / 3 derive their scaling from the operand extent they are given, so each tile gets its own); its
+ *      device budget is the option "stream_budget_mb" (0 = free device memory at the call minus 1 GiB).  Every other operator
+ *      fails with MR_ENOTSUP on a host-resident operand: call mr_matrix_to_device first.  Sharded datasets stay device-only. */
+MR_API mr_status mr_matrix_create_host(mr_context* ctx, mr_matrix** out);
+/* *out = 1 iff m is host-resident */
+MR_API mr_status mr_matrix_is_host(const mr_matrix* m, int32_t* out);
+/* Copies between the residences; ids, shapes, formats and isTransposed flags are kept.  to_host copies on the egress stream after
+ * each block's producer; to_device copies on the ingest stream with an event and an ingest number per block (as put_block), so a
+ * multiply can start while the copy runs.  A dataset already in the target residence gives a new handle sharing its blocks. */
+/* to_host reads the device arrays asynchronously; arrays the library owns are released only after those reads, arrays a caller lent
+ * (mr_matrix_put_block_device) must stay valid until mr_sync. */
+MR_API mr_status mr_matrix_to_host(mr_matrix* m, mr_matrix** out);
+MR_API mr_status mr_matrix_to_device(mr_matrix* m, mr_matrix** out);
 
 /* ---- operators: argument-for-argument with M/Dataset.scala:57-152 and the physical operators
  *      of M/execution/MatfastExecution.scala. */
@@ -349,6 +369,9 @@ typedef struct mr_stats {
   int64_t tc_int8_ops;      /* int8 multiply-add operations (x 2) of the most recent tensor-core multiply */
   int64_t p2p_bytes;        /* bytes pulled from peer GPUs over NVLink by this context (grid multiply) */
   int64_t tc_moduli;        /* residue moduli of the most recent tensor-core (Ozaki-II) multiply */
+  int64_t stream_tiles;     /* C tiles of the most recent streamed multiply (a host-resident operand; mr_matrix_create_host) */
+  int64_t stream_h2d_bytes; /* operand panels that multiply moved host -> device (h2d_bytes also counts its descriptor tables) */
+  int64_t stream_d2h_bytes; /* result blocks that multiply moved device -> host */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

@@ -43,6 +43,8 @@ struct SparseMatrix {
   bool isTransposed = false;
 };
 
+class Dataset;
+
 class MatfastSession {
  public:
   explicit MatfastSession(int device = -1, bool compat_bugs = true, void* stream = nullptr) {
@@ -59,12 +61,16 @@ class MatfastSession {
   MatfastSession& operator=(const MatfastSession&) = delete;
   void sync() { check(mr_sync(ctx_)); }
   mr_context* raw() const { return ctx_; }
+  // an empty host-resident dataset (blocks in page-locked host memory); defined after Dataset
+  Dataset createHostDataset();
 
  private:
   mr_context* ctx_ = nullptr;
 };
 
 class Dataset {
+  friend class MatfastSession;
+
  public:
   explicit Dataset(MatfastSession& s) : session_(&s) {
     mr_matrix* h = nullptr;
@@ -95,6 +101,22 @@ class Dataset {
     d.valuesLen = static_cast<int64_t>(m.values.size());
     d.isTransposed = m.isTransposed;
     check(mr_matrix_put_block(h_.get(), rid, cid, &d));
+  }
+  // host residence: blocks in page-locked host memory; matrixMultiply streams such operands through the device
+  bool isHost() const {
+    int32_t host = 0;
+    check(mr_matrix_is_host(h_.get(), &host));
+    return host != 0;
+  }
+  Dataset toHost() const {
+    mr_matrix* o = nullptr;
+    check(mr_matrix_to_host(h_.get(), &o));
+    return Dataset(*session_, o);
+  }
+  Dataset toDevice() const {
+    mr_matrix* o = nullptr;
+    check(mr_matrix_to_device(h_.get(), &o));
+    return Dataset(*session_, o);
   }
   bool hasBlock(int32_t rid, int32_t cid) const {
     int32_t present = 0;
@@ -202,6 +224,12 @@ class Dataset {
   MatfastSession* session_;
   std::shared_ptr<mr_matrix> h_;
 };
+
+inline Dataset MatfastSession::createHostDataset() {
+  mr_matrix* h = nullptr;
+  check(mr_matrix_create_host(ctx_, &h));
+  return Dataset(*this, h);
+}
 
 // ---- one process, all GPUs of the box (mr_init_grid): the placement grid replaces the Spark cluster --------------------------
 class GridSession {

@@ -72,6 +72,9 @@ class mr_stats(C.Structure):
         ("tc_int8_ops", C.c_int64),
         ("p2p_bytes", C.c_int64),
         ("tc_moduli", C.c_int64),
+        ("stream_tiles", C.c_int64),
+        ("stream_h2d_bytes", C.c_int64),
+        ("stream_d2h_bytes", C.c_int64),
     ]
 
 
@@ -114,6 +117,10 @@ SIGNATURES = {
     "mr_matrix_block_ids": [_P, C.POINTER(_i32), C.POINTER(_i32), _i64],
     "mr_matrix_get_block": [_P, _i32, _i32, C.POINTER(mr_block_desc)],
     "mr_matrix_block_device_ptr": [_P, _i32, _i32, _PP],
+    "mr_matrix_create_host": [_P, _PP],
+    "mr_matrix_is_host": [_P, C.POINTER(_i32)],
+    "mr_matrix_to_host": [_P, _PP],
+    "mr_matrix_to_device": [_P, _PP],
     "mr_matrix_rand": [_P, _i64, _i64, _i32, _i64, _PP],
     "mr_matrix_sprand": [_P, _i64, _i64, _i32, _f64, _i64, C.c_uint8, _PP],
     "mr_matrix_rand_partition": [_P, _i64, _i64, _i32, _i64, _i32, _i32, _i32, _i32, _P, _i64, _PP],

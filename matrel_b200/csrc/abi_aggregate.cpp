@@ -9,6 +9,7 @@ extern "C" {
 static mr_status aggregate_operator(int op, mr_matrix* a, int64_t nrows, int64_t ncols, mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(a && out, MR_EINVAL, "null argument");
+    require_device(a, op == AGG_ROW_SUM ? "mr_row_sum" : op == AGG_COL_SUM ? "mr_col_sum" : op == AGG_SUM ? "mr_sum" : "mr_trace");
     if (op == AGG_TRACE)  // Dataset.scala:80
       MR_REQUIRE(nrows == ncols, MR_EDIM, "Cannot perform trace() on a rectangle matrix");
     mr_context* ctx = a->ctx;
@@ -97,6 +98,7 @@ mr_status mr_trace(mr_matrix* a, int64_t nrows, int64_t ncols, mr_matrix** out) 
 
 static mr_status slice_operator(mr_matrix* a, int32_t blkSize, bool take_row, int64_t index, int64_t index2, mr_matrix** out) {
   return guarded([&] {
+    require_device(a, index2 >= 0 ? "mr_selection" : "mr_project");
     MR_REQUIRE(blkSize > 0, MR_EINVAL, "blkSize must be positive, got %d", blkSize);
     mr_context* ctx = a->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
@@ -186,6 +188,7 @@ mr_status mr_vec(mr_matrix* a, int64_t nrows, int64_t ncols, int32_t blkSize, mr
   mr_status st = guarded([&] {
     MR_REQUIRE(a && out, MR_EINVAL, "null argument");
     MR_REQUIRE(blkSize > 0 && nrows > 0, MR_EINVAL, "nrows and blkSize must be positive");
+    require_device(a, "mr_vec");
   });
   if (st != MR_OK) return st;
   st = mr_materialize(a, &canon);  // column-major, non-transposed dense blocks (shares already canonical ones)

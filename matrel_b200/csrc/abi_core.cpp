@@ -248,6 +248,68 @@ void validate_desc(const mr_block_desc* d) {
   }
 }
 
+void require_device(const mr_matrix* m, const char* op) {
+  if (m && m->host)
+    fail(MR_ENOTSUP, "%s: the dataset is host-resident; only mr_matrix_multiply streams host-resident operands, call "
+                     "mr_matrix_to_device first", op);
+}
+
+// Host-resident datasets grow chunk by chunk: 2 MiB first, then as large as the store already is, up to 1 GiB.
+constexpr size_t kPinnedChunkMin = 2u << 20, kPinnedChunkMax = 1u << 30;
+
+Span HostStore::take(size_t bytes) {
+  const size_t need = align_up(std::max<size_t>(bytes, 16));
+  if (chunks.empty() || used + need > chunks.back().second) {
+    const size_t want = std::max(need, std::min(kPinnedChunkMax, std::max(kPinnedChunkMin, total)));
+    void* p = nullptr;
+    size_t got = 0;
+    {
+      std::lock_guard<std::mutex> g(ctx->pinned_mu);
+      auto it = ctx->pinned_free.lower_bound(want);
+      if (it != ctx->pinned_free.end() && it->first <= 4 * want) {
+        p = it->second;
+        got = it->first;
+        ctx->pinned_free.erase(it);
+      }
+    }
+    if (!p) {
+      cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
+      if (e != cudaSuccess) {  // hand the cached chunks back to the system and try once more
+        (void)cudaGetLastError();
+        {
+          std::lock_guard<std::mutex> g(ctx->pinned_mu);
+          for (auto& kv : ctx->pinned_free) cudaFreeHost(kv.second);
+          ctx->pinned_free.clear();
+        }
+        e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
+        if (e != cudaSuccess) {
+          (void)cudaGetLastError();
+          fail(MR_ENOMEM, "cudaHostAlloc(%zu bytes) of page-locked memory for a host-resident dataset failed: %s", want,
+               cudaGetErrorString(e));
+        }
+      }
+      got = want;
+    }
+    chunks.emplace_back(p, got);
+    total += got;
+    used = 0;
+  }
+  void* w = static_cast<char*>(chunks.back().first) + used;
+  used += need;
+  return Span{std::make_shared<DevBuf>(ctx, w, bytes), 0};
+}
+
+HostStore::~HostStore() {
+  if (chunks.empty()) return;
+  // copies to and from these chunks run on the ingest / egress streams: they must be done before the memory is reused
+  cudaStreamSynchronize(ctx->h2d_stream);
+  cudaStreamSynchronize(ctx->d2h_stream);
+  cudaStreamSynchronize(ctx->stream);
+  (void)cudaGetLastError();
+  std::lock_guard<std::mutex> g(ctx->pinned_mu);
+  for (auto& c : chunks) ctx->pinned_free.emplace(c.second, c.first);
+}
+
 Span upload_raw(mr_context* ctx, const void* host, size_t bytes) {
   Span s{std::make_shared<DevBuf>(ctx, std::max<size_t>(bytes, 16)), 0};
   if (bytes) {
@@ -358,6 +420,7 @@ mr_status mr_shutdown(mr_context* ctx) {
       if (ctx->chunk_join[i]) cudaEventDestroy(ctx->chunk_join[i]);
     }
     if (ctx->stage_host) cudaFreeHost(ctx->stage_host);
+    for (auto& kv : ctx->pinned_free) cudaFreeHost(kv.second);
     if (ctx->ev_alloc) cudaEventDestroy(ctx->ev_alloc);
     if (ctx->ev_order) cudaEventDestroy(ctx->ev_order);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -409,6 +472,10 @@ mr_status mr_set_option(mr_context* ctx, const char* key, int64_t value) {
     else if (k == "gemm_variant") ctx->force_variant = static_cast<int>(value);
     else if (k == "oz2_ksplit") ctx->oz2_ksplit = static_cast<int>(value);
     else if (k == "pipeline") ctx->pipeline = static_cast<int>(value);
+    else if (k == "stream_budget_mb") {
+      MR_REQUIRE(value >= 0, MR_EINVAL, "stream_budget_mb must be >= 0, got %lld", (long long)value);
+      ctx->stream_budget_mb = value;
+    }
     else fail(MR_EINVAL, "unknown option '%s'", key);
   });
 }
@@ -471,6 +538,145 @@ mr_status mr_matrix_create(mr_context* ctx, mr_matrix** out) {
   });
 }
 
+mr_status mr_matrix_create_host(mr_context* ctx, mr_matrix** out) {
+  return guarded([&] {
+    MR_REQUIRE(ctx != nullptr && out != nullptr, MR_EINVAL, "ctx/out is null");
+    std::unique_ptr<mr_matrix> m(new_matrix(ctx));
+    m->host = std::make_shared<HostStore>(ctx);
+    *out = m.release();
+  });
+}
+
+mr_status mr_matrix_is_host(const mr_matrix* m, int32_t* out) {
+  return guarded([&] {
+    MR_REQUIRE(m != nullptr && out != nullptr, MR_EINVAL, "matrix/out is null");
+    *out = m->host ? 1 : 0;
+  });
+}
+
+// Device -> host: every block is copied on the egress stream after its own producer; the copies' completion event becomes
+// the host blocks' `ready`, so readers (mr_matrix_get_block, mr_matrix_to_device, a streamed multiply) wait for exactly them.
+mr_status mr_matrix_to_host(mr_matrix* m, mr_matrix** out) {
+  return guarded([&] {
+    MR_REQUIRE(m != nullptr && out != nullptr, MR_EINVAL, "matrix/out is null");
+    mr_context* ctx = m->ctx;
+    DeviceScope dev(ctx);
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    std::unique_ptr<mr_matrix> r(new_matrix(ctx));
+    if (m->host) {  // already host-resident: the new handle shares the store (datasets are immutable)
+      r->host = m->host;
+      r->blocks = m->blocks;
+      r->temps = m->temps;
+      *out = r.release();
+      return;
+    }
+    r->host = std::make_shared<HostStore>(ctx);
+    cudaStream_t rs = ctx->pipeline ? ctx->d2h_stream : ctx->stream;
+    if (rs != ctx->stream) {  // blocks without an event of their own were produced on the context stream
+      CUDA_CHECK(cudaEventRecord(ctx->ev_order, ctx->stream));
+      CUDA_CHECK(cudaStreamWaitEvent(rs, ctx->ev_order, 0));
+    }
+    auto copy_out = [&](const Span& src, size_t bytes) {
+      Span h = r->host->take(bytes);
+      if (bytes) {
+        CUDA_CHECK(cudaMemcpyAsync(h.buf->p, src.ptr<char>(), bytes, cudaMemcpyDeviceToHost, rs));
+        ctx->stats.d2h_bytes += static_cast<int64_t>(bytes);
+      }
+      return h;
+    };
+    for (auto& kv : m->blocks) {
+      const Block& b = kv.second;
+      wait_ready_on(rs, b);
+      Block h = b;
+      h.ready.reset();
+      h.seq = 0;
+      h.settled = false;
+      h.values = copy_out(b.values, static_cast<size_t>(b.valuesLen) * sizeof(double));
+      if (!b.dense()) {
+        h.colPtrs = copy_out(b.colPtrs, static_cast<size_t>(b.colPtrsLen) * sizeof(int32_t));
+        h.rowIndices = copy_out(b.rowIndices, static_cast<size_t>(b.valuesLen) * sizeof(int32_t));
+      }
+      r->blocks[kv.first] = std::move(h);
+    }
+    // The source's device arrays are released on the context stream (when the source is freed, possibly right after this call):
+    // that free must wait for the copies reading them.  `done` replaces each array's own release event, so it is recorded after it.
+    std::vector<DevBuf*> sources;
+    if (rs != ctx->stream)
+      for (auto& kv : m->blocks)
+        for (const Span* sp : {&kv.second.values, &kv.second.colPtrs, &kv.second.rowIndices})
+          if (sp->buf && sp->buf->owned && !sp->buf->sync_alloc) {
+            if (sp->buf->ready) CUDA_CHECK(cudaStreamWaitEvent(rs, sp->buf->ready->ev, 0));
+            sources.push_back(sp->buf.get());
+          }
+    ReadyPtr done = std::make_shared<Ready>();
+    CUDA_CHECK(cudaEventRecord(done->ev, rs));
+    for (auto& kv : r->blocks) kv.second.ready = done;
+    for (DevBuf* b : sources) b->ready = done;
+    *out = r.release();
+  });
+}
+
+// Host -> device on the ingest stream, with an event and an ingest sequence number per block like mr_matrix_put_block: a
+// multiply can start on the blocks that have landed.
+mr_status mr_matrix_to_device(mr_matrix* m, mr_matrix** out) {
+  return guarded([&] {
+    MR_REQUIRE(m != nullptr && out != nullptr, MR_EINVAL, "matrix/out is null");
+    mr_context* ctx = m->ctx;
+    DeviceScope dev(ctx);
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    std::unique_ptr<mr_matrix> r(new_matrix(ctx));
+    if (!m->host) {  // already device-resident: the new handle shares the device arrays, and a sharded dataset's layout
+      r->blocks = m->blocks;
+      r->shard = m->shard;
+      r->temps = m->temps;
+      *out = r.release();
+      return;
+    }
+    size_t total = 0;
+    for (auto& kv : m->blocks) {
+      const Block& b = kv.second;
+      total += align_up(static_cast<size_t>(b.valuesLen) * sizeof(double));
+      if (!b.dense()) total += align_up(static_cast<size_t>(b.colPtrsLen) * 4) + align_up(static_cast<size_t>(b.valuesLen) * 4);
+    }
+    Slab slab(ctx, total);
+    cudaStream_t cs = ctx->pipeline ? ctx->h2d_stream : ctx->stream;
+    if (ctx->pipeline) {  // the slab is allocated on the context stream: the ingest stream must see it
+      CUDA_CHECK(cudaEventRecord(ctx->ev_alloc, ctx->stream));
+      CUDA_CHECK(cudaStreamWaitEvent(cs, ctx->ev_alloc, 0));
+    }
+    auto copy_in = [&](const Span& src, size_t bytes) {
+      Span d = slab.take(bytes);
+      if (bytes) {
+        CUDA_CHECK(cudaMemcpyAsync(d.ptr<char>(), src.buf->p, bytes, cudaMemcpyHostToDevice, cs));
+        ctx->stats.h2d_bytes += static_cast<int64_t>(bytes);
+      }
+      return d;
+    };
+    ReadyPtr last;
+    for (auto& kv : m->blocks) {
+      const Block& b = kv.second;
+      if (b.ready) CUDA_CHECK(cudaStreamWaitEvent(cs, b.ready->ev, 0));  // the host block is still being written back
+      Block d = b;
+      d.ready.reset();
+      d.settled = false;
+      d.values = copy_in(b.values, static_cast<size_t>(b.valuesLen) * sizeof(double));
+      if (!b.dense()) {
+        d.colPtrs = copy_in(b.colPtrs, static_cast<size_t>(b.colPtrsLen) * sizeof(int32_t));
+        d.rowIndices = copy_in(b.rowIndices, static_cast<size_t>(b.valuesLen) * sizeof(int32_t));
+      }
+      if (ctx->pipeline) {
+        last = std::make_shared<Ready>();
+        CUDA_CHECK(cudaEventRecord(last->ev, cs));
+        d.ready = last;
+        d.seq = ++ctx->ingest_seq;
+      }
+      r->blocks[kv.first] = std::move(d);
+    }
+    slab.buf->ready = last;  // the ingest stream is in order: the last copy's event covers every copy into the slab
+    *out = r.release();
+  });
+}
+
 mr_status mr_matrix_free(mr_matrix* m) {
   return guarded([&] {
     if (!m) return;
@@ -526,6 +732,21 @@ mr_status mr_matrix_put_block(mr_matrix* m, int32_t rid, int32_t cid, const mr_b
     b.numCols = d->numCols;
     b.isT = d->isTransposed != 0;
     b.valuesLen = d->valuesLen;
+    if (m->host) {  // copied into the dataset's page-locked store: the caller's arrays are free when the call returns
+      auto copy_in = [&](const void* src, size_t bytes) {
+        Span s = m->host->take(bytes);
+        if (bytes) std::memcpy(s.buf->p, src, bytes);
+        return s;
+      };
+      b.values = copy_in(d->values, static_cast<size_t>(d->valuesLen) * sizeof(double));
+      if (d->type == 0) {
+        b.colPtrsLen = d->colPtrsLen;
+        b.colPtrs = copy_in(d->colPtrs, static_cast<size_t>(d->colPtrsLen) * sizeof(int32_t));
+        b.rowIndices = copy_in(d->rowIndices, static_cast<size_t>(d->rowIndicesLen) * sizeof(int32_t));
+      }
+      m->blocks[{rid, cid}] = std::move(b);
+      return;
+    }
     // Ingest on its own stream: the copy of block k+1 overlaps whatever the context stream is computing, and
     // operators wait per block (Block::ready), so a multiply can start on the row panels that have landed.
     cudaStream_t cs = ctx->pipeline ? ctx->h2d_stream : ctx->stream;
@@ -605,6 +826,7 @@ mr_status mr_matrix_put_block_device(mr_matrix* m, int32_t rid, int32_t cid, int
     MR_REQUIRE(m != nullptr, MR_EINVAL, "matrix is null");
     MR_REQUIRE(numRows >= 0 && numCols >= 0, MR_EINVAL, "negative block dimensions %d x %d", numRows, numCols);
     MR_REQUIRE(dvalues != nullptr || static_cast<int64_t>(numRows) * numCols == 0, MR_EINVAL, "device pointer is null");
+    require_device(m, "mr_matrix_put_block_device");
     Span s{std::make_shared<DevBuf>(m->ctx, const_cast<double*>(dvalues),
                                     static_cast<size_t>(numRows) * numCols * sizeof(double)),
            0};
@@ -618,6 +840,7 @@ mr_status mr_matrix_put_blocks_device(mr_matrix* m, int64_t count, const int32_t
   return guarded([&] {
     MR_REQUIRE(m != nullptr, MR_EINVAL, "matrix is null");
     MR_REQUIRE(count == 0 || (rids && cids && numRows && numCols && dvalues), MR_EINVAL, "null argument");
+    require_device(m, "mr_matrix_put_blocks_device");
     for (int64_t i = 0; i < count; ++i) {
       MR_REQUIRE(numRows[i] >= 0 && numCols[i] >= 0, MR_EINVAL, "negative block dimensions %d x %d", numRows[i], numCols[i]);
       Span s{std::make_shared<DevBuf>(m->ctx, const_cast<double*>(dvalues[i]),
@@ -675,7 +898,10 @@ mr_status mr_matrix_get_block(mr_matrix* m, int32_t rid, int32_t cid, mr_block_d
     // Egress on its own stream, ordered after this block's producer only (one chunk of a chunked multiply, or
     // everything enqueued on the context stream so far when the block has no event of its own).
     cudaStream_t rs = ctx->pipeline ? ctx->d2h_stream : ctx->stream;
-    if (ctx->pipeline && (io->values || io->colPtrs || io->rowIndices)) {
+    const bool host = m->host != nullptr, any = io->values || io->colPtrs || io->rowIndices;
+    if (host) {  // page-locked host memory: only a write-back still in flight (the block's event) has to be waited for
+      if (ready && any) CUDA_CHECK(cudaEventSynchronize(ready->ev));
+    } else if (ctx->pipeline && any) {
       if (ready) {
         CUDA_CHECK(cudaStreamWaitEvent(rs, ready->ev, 0));
       } else if (!settled) {
@@ -683,28 +909,29 @@ mr_status mr_matrix_get_block(mr_matrix* m, int32_t rid, int32_t cid, mr_block_d
         CUDA_CHECK(cudaStreamWaitEvent(rs, ctx->ev_order, 0));
       }
     }
+    auto copy = [&](void* dst, const void* src, int64_t bytes) {
+      if (bytes <= 0) return;
+      if (host) {
+        std::memcpy(dst, src, static_cast<size_t>(bytes));
+      } else {
+        CUDA_CHECK(cudaMemcpyAsync(dst, src, static_cast<size_t>(bytes), cudaMemcpyDeviceToHost, rs));
+        ctx->stats.d2h_bytes += bytes;
+      }
+    };
     if (io->values != nullptr) {
       MR_REQUIRE(io->valuesLen >= b.valuesLen, MR_EINVAL, "values capacity %lld < %lld", (long long)io->valuesLen,
                  (long long)b.valuesLen);
-      if (b.valuesLen)
-        CUDA_CHECK(cudaMemcpyAsync(io->values, b.values.ptr<double>(), static_cast<size_t>(b.valuesLen) * sizeof(double),
-                                   cudaMemcpyDeviceToHost, rs));
-      ctx->stats.d2h_bytes += b.valuesLen * 8;
+      copy(io->values, b.values.ptr<double>(), b.valuesLen * 8);
     }
     if (!b.dense() && io->colPtrs != nullptr) {
       MR_REQUIRE(io->colPtrsLen >= b.colPtrsLen, MR_EINVAL, "colPtrs capacity too small");
-      CUDA_CHECK(cudaMemcpyAsync(io->colPtrs, b.colPtrs.ptr<int32_t>(), static_cast<size_t>(b.colPtrsLen) * 4,
-                                 cudaMemcpyDeviceToHost, rs));
-      ctx->stats.d2h_bytes += b.colPtrsLen * 4;
+      copy(io->colPtrs, b.colPtrs.ptr<int32_t>(), b.colPtrsLen * 4);
     }
     if (!b.dense() && io->rowIndices != nullptr) {
       MR_REQUIRE(io->rowIndicesLen >= rowIndicesLen, MR_EINVAL, "rowIndices capacity too small");
-      if (rowIndicesLen)
-        CUDA_CHECK(cudaMemcpyAsync(io->rowIndices, b.rowIndices.ptr<int32_t>(), static_cast<size_t>(rowIndicesLen) * 4,
-                                   cudaMemcpyDeviceToHost, rs));
-      ctx->stats.d2h_bytes += rowIndicesLen * 4;
+      copy(io->rowIndices, b.rowIndices.ptr<int32_t>(), rowIndicesLen * 4);
     }
-    if (io->values || io->colPtrs || io->rowIndices) CUDA_CHECK(cudaStreamSynchronize(rs));
+    if (any && !host) CUDA_CHECK(cudaStreamSynchronize(rs));
     io->type = b.type;
     io->numRows = b.numRows;
     io->numCols = b.numCols;
@@ -718,6 +945,7 @@ mr_status mr_matrix_get_block(mr_matrix* m, int32_t rid, int32_t cid, mr_block_d
 mr_status mr_matrix_block_device_ptr(mr_matrix* m, int32_t rid, int32_t cid, double** dptr) {
   return guarded([&] {
     MR_REQUIRE(m != nullptr && dptr != nullptr, MR_EINVAL, "null argument");
+    require_device(m, "mr_matrix_block_device_ptr");
     auto it = m->blocks.find({rid, cid});
     if (it == m->blocks.end()) fail(MR_ENOTFOUND, "no block (%d, %d) in this dataset", rid, cid);
     *dptr = it->second.values.ptr<double>();

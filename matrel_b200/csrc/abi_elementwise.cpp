@@ -166,6 +166,7 @@ extern "C" {
 mr_status mr_transpose(mr_matrix* a, mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(a && out, MR_EINVAL, "null argument");
+    require_device(a, "mr_transpose");
     std::unique_ptr<mr_matrix> r(new_matrix(a->ctx));
     for (auto& kv : a->blocks) {
       Block b = kv.second;  // shares the device arrays (DenseMatrix.transpose, MLMatrix.scala:312; Sparse :634-635)
@@ -181,6 +182,9 @@ static mr_status ew_operator(int op, mr_matrix* left, int64_t lr, int64_t lc, mr
                              mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(left && right && out, MR_EINVAL, "null argument");
+    const char* name = op == EW_ADD ? "mr_add_element" : op == EW_MUL ? "mr_multiply_element" : "mr_divide_element";
+    require_device(left, name);
+    require_device(right, name);
     MR_REQUIRE(left->ctx == right->ctx, MR_EINVAL, "operands belong to different contexts");
     check_same_dims(lr, lc, rr, rc);
     std::lock_guard<std::mutex> lock(left->ctx->mu);
@@ -211,6 +215,7 @@ mr_status mr_divide_element(mr_matrix* left, int64_t lr, int64_t lc, mr_matrix* 
 static mr_status map_operator(int op, mr_matrix* a, double alpha, mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(a && out, MR_EINVAL, "null argument");
+    require_device(a, op == MAP_ADD_SCALAR ? "mr_add_scalar" : op == MAP_MUL_SCALAR ? "mr_multiply_scalar" : "mr_power");
     std::lock_guard<std::mutex> lock(a->ctx->mu);
     wait_ready_all(a->ctx, a);
     std::unique_ptr<mr_matrix> r(new_matrix(a->ctx));
@@ -227,6 +232,8 @@ mr_status mr_rank_one_update(mr_matrix* left, int64_t lr, int64_t lc, mr_matrix*
   (void)blkSize;
   return guarded([&] {
     MR_REQUIRE(left && right && out, MR_EINVAL, "null argument");
+    require_device(left, "mr_rank_one_update");
+    require_device(right, "mr_rank_one_update");
     MR_REQUIRE(left->ctx == right->ctx, MR_EINVAL, "operands belong to different contexts");
     mr_context* ctx = left->ctx;
     if (ctx->compat_bugs) {
@@ -287,6 +294,7 @@ mr_status mr_rank_one_update(mr_matrix* left, int64_t lr, int64_t lc, mr_matrix*
 mr_status mr_materialize(mr_matrix* a, mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(a && out, MR_EINVAL, "null argument");
+    require_device(a, "mr_materialize");
     mr_context* ctx = a->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     wait_ready_all(ctx, a);

@@ -216,6 +216,8 @@ static mr_status grid_multiply_impl(mr_matrix* A, mr_matrix* B, const double* co
                                     int32_t nchunks, const void* const* gates, mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(A && B && out && slabsA_row && slabsB_col, MR_EINVAL, "null argument");
+    require_device(A, "mr_grid_multiply");
+    require_device(B, "mr_grid_multiply");
     MR_REQUIRE(A->shard && B->shard, MR_EINVAL, "operands must be sharded datasets (mr_matrix_create_sharded)");
     MR_REQUIRE(A->ctx == B->ctx, MR_EINVAL, "operands belong to different contexts");
     const ShardLayout LA = A->shard->L, LB = B->shard->L;
@@ -370,6 +372,7 @@ mr_status mr_grid_multiply_gated(mr_matrix* A, mr_matrix* B, const double* const
 mr_status mr_matrix_filter_blocks(mr_matrix* a, int32_t row_mod, int32_t row_rem, int32_t col_mod, int32_t col_rem, mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(a && out, MR_EINVAL, "null argument");
+    require_device(a, "mr_matrix_filter_blocks");
     MR_REQUIRE(row_mod >= 1 && col_mod >= 1 && row_rem >= 0 && row_rem < row_mod && col_rem >= 0 && col_rem < col_mod, MR_EINVAL,
                "bad partition (%d mod %d, %d mod %d)", row_rem, row_mod, col_rem, col_mod);
     std::lock_guard<std::mutex> lock(a->ctx->mu);
@@ -388,6 +391,7 @@ mr_status mr_grid_multiply_rows(mr_matrix* A_rows, int64_t leftRowNum, int64_t l
                                 mr_matrix** out) {
   return guarded([&] {
     MR_REQUIRE(A_rows && B && out && slabsB_col, MR_EINVAL, "null argument");
+    require_device(A_rows, "mr_grid_multiply_rows");
     MR_REQUIRE(B->shard, MR_EINVAL, "the right operand must be a sharded dataset (mr_matrix_create_sharded)");
     MR_REQUIRE(A_rows->ctx == B->ctx, MR_EINVAL, "operands belong to different contexts");
     const ShardLayout LB = B->shard->L;

@@ -25,6 +25,18 @@ struct OutPlan {
   std::vector<std::pair<const Block*, const Block*>> spsp;  // sparse x sparse, both densities <= 0.1 (ascending k)
 };
 
+// How LocalMatrix.matrixMultiplication computes one partial product a x b (LocalMatrix.scala:889-914)
+enum PairKind { PAIR_GEMM = 0, PAIR_SPMM = 1, PAIR_SPSP = 2 };
+int pair_kind(const Block& a, const Block& b) {
+  if (a.dense()) return PAIR_GEMM;  // dense x dense, dense x sparse.toDense (:891-892)
+  if (b.dense()) return PAIR_SPMM;  // sparse x dense (:893-899)
+  const double s1 = a.valuesLen * 1.0 / (static_cast<double>(a.numRows) * a.numCols);
+  const double s2 = b.valuesLen * 1.0 / (static_cast<double>(b.numRows) * b.numCols);
+  if (s1 > 0.1) return PAIR_GEMM;   // :903-904
+  if (s2 > 0.1) return PAIR_SPMM;   // :906-907
+  return PAIR_SPSP;                 // :909-911
+}
+
 struct MultiplyPlanner {
   mr_context* ctx;
   std::deque<Block> temps;   // densified sparse operands kept alive until the launches are enqueued (deque: the
@@ -57,20 +69,13 @@ struct MultiplyPlanner {
                  "Matrix A and B must have the same number of cols. But found A.numCols = %d, B.numCols = %d", o.n,
                  b.numCols);
     }
-    if (a.dense()) {
-      push_gemm(o, a, dense_of(b), k);  // dense x dense, dense x sparse.toDense (:891-892)
-    } else if (b.dense()) {
-      o.spmm.emplace_back(&a, &b);   // sparse x dense (:893-899; the n == 1 SpMV case is the same kernel)
+    const int kind = pair_kind(a, b);
+    if (kind == PAIR_GEMM) {
+      push_gemm(o, dense_of(a), dense_of(b), k);
+    } else if (kind == PAIR_SPMM) {
+      o.spmm.emplace_back(&a, &dense_of(b));  // the n == 1 SpMV case is the same kernel
     } else {
-      const double s1 = a.valuesLen * 1.0 / (static_cast<double>(a.numRows) * a.numCols);
-      const double s2 = b.valuesLen * 1.0 / (static_cast<double>(b.numRows) * b.numCols);
-      if (s1 > 0.1) {
-        push_gemm(o, dense_of(a), dense_of(b), k);  // :903-904
-      } else if (s2 > 0.1) {
-        o.spmm.emplace_back(&a, &dense_of(b));   // :906-907
-      } else {
-        o.spsp.emplace_back(&a, &b);  // LocalMatrix.multiplySparseSparse (:909-911, :143-323): see run_sparse_chains
-      }
+      o.spsp.emplace_back(&a, &b);  // LocalMatrix.multiplySparseSparse (:909-911, :143-323): see run_sparse_chains
     }
   }
 
@@ -170,6 +175,31 @@ bool try_ozaki(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<d
   return true;
 }
 
+// The largest (row panel x column panel) job grid cap_r x cap_c of an nr x nc grid of output blocks whose residue scratch fits the
+// ozaki_scratch_mb budget (0 = 16 GiB), halving the longer side first.  Returns false when not even 1 x 1 fits.  `bytes`: that
+// scratch (an upper bound of what oz2_create allocates).
+bool oz2_capacity(const mr_context* ctx, int32_t blk, int64_t K, int T, int nr, int nc, int& cap_r, int& cap_c, size_t* bytes = nullptr) {
+  const int ss = (blk + kOz2TileM - 1) / kOz2TileM * kOz2TileM;
+  auto panel_tiles = [&](int ncr, int ncc) {  // upper bound of a panel's tile count
+    const int64_t tm = static_cast<int64_t>(ncr) * (ss / kOz2TileM);
+    const int64_t tn = (static_cast<int64_t>(ncc) * ss + kOz2TileN - 1) / kOz2TileN;
+    return tm * tn;
+  };
+  const int64_t plane_cap_tiles = std::max<int64_t>(64, (2ll << 30) / (static_cast<int64_t>(T) * kOz2TileM * kOz2TileN));
+  const size_t budget = static_cast<size_t>(ctx->ozaki_scratch_mb > 0 ? ctx->ozaki_scratch_mb : 16384) << 20;
+  cap_r = nr;
+  cap_c = nc;
+  auto max_tiles_for = [&](int r, int cc_) { return static_cast<int>(std::min<int64_t>(plane_cap_tiles, panel_tiles(r, cc_))); };
+  size_t need;
+  while ((need = oz2_scratch_bytes(blk, K, T, cap_r, cap_c, max_tiles_for(cap_r, cap_c))) > budget) {
+    if (cap_r == 1 && cap_c == 1) return false;
+    if (cap_r >= cap_c) cap_r = (cap_r + 1) / 2;
+    else cap_c = (cap_c + 1) / 2;
+  }
+  if (bytes) *bytes = need;
+  return true;
+}
+
 // ------------------------------------------------------------------------------------------------
 // gemm_algo 0 (auto) / 4: the dense pairs through the Ozaki-II job engine (gemm_ozaki.cu), group by group.
 //
@@ -264,21 +294,8 @@ struct Oz2Run {
       }
     }
     // ---- capacity: everything resident, or (row panel x column panel) jobs within the scratch budget
-    auto panel_tiles = [&](int ncr, int ncc) {  // upper bound of a panel's tile count
-      const int64_t tm = static_cast<int64_t>(ncr) * (ss / kOz2TileM);
-      const int64_t tn = (static_cast<int64_t>(ncc) * ss + kOz2TileN - 1) / kOz2TileN;
-      return tm * tn;
-    };
     const int64_t plane_cap_tiles = std::max<int64_t>(64, (2ll << 30) / (static_cast<int64_t>(T) * kOz2TileM * kOz2TileN));
-    const size_t budget = static_cast<size_t>(ctx->ozaki_scratch_mb > 0 ? ctx->ozaki_scratch_mb : 16384) << 20;
-    cap_r = nr;
-    cap_c = nc;
-    auto max_tiles_for = [&](int r, int cc_) { return static_cast<int>(std::min<int64_t>(plane_cap_tiles, panel_tiles(r, cc_))); };
-    while (oz2_scratch_bytes(blk, K, T, cap_r, cap_c, max_tiles_for(cap_r, cap_c)) > budget) {
-      if (cap_r == 1 && cap_c == 1) return false;
-      if (cap_r >= cap_c) cap_r = (cap_r + 1) / 2;
-      else cap_c = (cap_c + 1) / 2;
-    }
+    if (!oz2_capacity(ctx, blk, K, T, nr, nc, cap_r, cap_c)) return false;
     const bool resident = cap_r == nr && cap_c == nc;
     if (!resident) {  // panels re-prepare their slots: one group, after every operand has landed
       std::fill(group_of.begin(), group_of.end(), 0);
@@ -611,7 +628,8 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
 }
 
 void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner& planner, int32_t blkSize,
-                  mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows) {
+                  mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows,
+                  const MultiplyDecisions* decisions) {
   const ShardInfo* out_shard = result->shard.get();
   // Low-density sparse x sparse pairs: next to any dense partial the block sum is dense whatever the partial's own format
   // (LocalMatrix.add), so there they are ordinary sparse x dense products of the densified right operand; an output block
@@ -713,6 +731,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     int64_t tiles128 = 0;
     for (auto& go : outs) tiles128 += static_cast<int64_t>((go.m + 127) / 128) * ((go.n + 127) / 128);
     int variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
+    if (decisions) variant = decisions->variant;
     if (ctx->force_variant >= 0) variant = ctx->force_variant;
     const int BM = gemm_tile_m(variant), BN = gemm_tile_n(variant);
     const int tpbm = std::max(1, (blkSize + BM - 1) / BM), tpbn = std::max(1, (blkSize + BN - 1) / BN);
@@ -772,7 +791,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     // when the engine's device flag reports operands it cannot represent.  Small products stay on the exact kernel in auto mode.
     Oz2Run oz2;
     bool use_oz2 = false;
-    if (algo == 4 || (algo == 0 && flops >= (1ll << 33)))
+    if (decisions ? decisions->oz2 : (algo == 4 || (algo == 0 && flops >= (1ll << 33))))
       use_oz2 = oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0);
     auto grp = [&](const Keyed& k) { return group_of[k.t.out]; };
     std::sort(keyed.begin(), keyed.end(), [&](const Keyed& x, const Keyed& y) {
@@ -1097,7 +1116,8 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
 namespace mrhost {
 
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
-                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows) {
+                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows,
+                         const MultiplyDecisions* decisions) {
   for (auto& kv : left->blocks)
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
   for (auto& kv : right->blocks)
@@ -1153,8 +1173,66 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
   std::unique_ptr<mr_matrix> result(out_layout ? new_sharded(ctx, *out_layout, false, false) : new_matrix(ctx));
   if (out_layout) result->blocks.clear();  // only the blocks the product has are present (join semantics); absent ones stay absent
   run_multiply(ctx, plans, planner, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, leftColBlkNum == 1 && rightRowBlkNum == 1,
-               out_windows);
+               out_windows, decisions);
   return result.release();
+}
+
+// The output blocks of left x right and their partial products, walked exactly as multiply_impl builds its plans (join on k in
+// ascending k, or the outer-product path with the last duplicate winning), but from metadata: no block is touched.
+MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, const mr_matrix* right, int64_t leftColNum,
+                                     int64_t rightRowNum, int32_t blkSize) {
+  struct Out {
+    int32_t m = 0, n = 0;
+    bool gemm = false, other = false;
+    int64_t flops = 0;
+  };
+  std::map<std::pair<int32_t, int32_t>, Out> outs;
+  auto pair_into = [](Out& o, const Block& a, const Block& b) {
+    o.m = a.numRows;
+    o.n = b.numCols;
+    if (pair_kind(a, b) == PAIR_GEMM) {
+      o.gemm = true;
+      o.flops += 2ll * a.numRows * b.numCols * a.numCols;
+    } else {
+      o.other = true;
+    }
+  };
+  if (ceil_div(leftColNum, blkSize) == 1 && ceil_div(rightRowNum, blkSize) == 1) {
+    for (auto& l : left->blocks)
+      for (auto& r : right->blocks) {
+        Out o;
+        pair_into(o, l.second, r.second);
+        outs[{l.first.first, r.first.second}] = o;
+      }
+  } else {
+    std::map<int32_t, std::vector<std::pair<int32_t, const Block*>>> rights;
+    for (auto& r : right->blocks) rights[r.first.first].push_back({r.first.second, &r.second});
+    for (auto& l : left->blocks) {
+      auto rit = rights.find(l.first.second);
+      if (rit == rights.end()) continue;
+      for (auto& jb : rit->second) pair_into(outs[{l.first.first, jb.first}], l.second, *jb.second);
+    }
+  }
+  int64_t flops = 0, tiles128 = 0;
+  bool mixed = false;
+  for (auto& kv : outs) {
+    const Out& o = kv.second;
+    if (!o.gemm || o.m == 0 || o.n == 0) continue;
+    flops += o.flops;
+    tiles128 += static_cast<int64_t>((o.m + 127) / 128) * ((o.n + 127) / 128);
+    mixed = mixed || o.other;  // a block with sparse partials next to dense ones keeps the whole product off the Ozaki-II engine
+  }
+  MultiplyDecisions d;
+  d.variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
+  d.oz2 = !mixed && (ctx->gemm_algo == 4 || (ctx->gemm_algo == 0 && flops >= (1ll << 33)));
+  return d;
+}
+
+size_t oz2_scratch_for(const mr_context* ctx, int32_t blk, int64_t K, int nr, int nc) {
+  if (K <= 0 || K >= (1 << 17) || nr <= 0 || nc <= 0) return 0;
+  int cap_r = 0, cap_c = 0;
+  size_t bytes = 0;
+  return oz2_capacity(ctx, blk, K, oz2_moduli_for(K, ctx->crt_moduli), nr, nc, cap_r, cap_c, &bytes) ? bytes : 0;
 }
 
 }  // namespace mrhost
@@ -1176,7 +1254,10 @@ mr_status mr_matrix_multiply(mr_matrix* left, int64_t leftRowNum, int64_t leftCo
     mr_context* ctx = left->ctx;
     DeviceScope dev(ctx);
     std::lock_guard<std::mutex> lock(ctx->mu);
-    *out = multiply_impl(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize, nullptr);
+    if (left->host || right->host)  // C tile by C tile through the device, into a host-resident result (abi_stream.cpp)
+      *out = multiply_streamed(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
+    else
+      *out = multiply_impl(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize, nullptr);
   });
 }
 

@@ -107,6 +107,10 @@ struct mr_context {
   int pipeline = 1;
   cudaStream_t p2p_stream = nullptr;             // pulls of peers' blocks over NVLink (copy engines), see abi_grid.cpp
   std::map<std::string, void*> ipc_open;         // CUDA IPC handles opened by this context (handle bytes -> mapped base)
+  int64_t stream_budget_mb = 0;  // device budget of a streamed multiply (0 = free device memory at the call minus 1 GiB)
+  // page-locked chunks of freed host-resident datasets, kept for the next one (pinning is slow); released by mr_shutdown
+  std::multimap<size_t, void*> pinned_free;
+  std::mutex pinned_mu;
   mr_stats stats{};
   std::mutex mu;
 };
@@ -128,7 +132,7 @@ using ReadyPtr = std::shared_ptr<Ready>;
 
 struct DevBuf {
   mr_context* ctx;
-  ReadyPtr ready;  // set when another stream writes this buffer: the free must be ordered after it
+  ReadyPtr ready;  // set when another stream writes or reads this buffer: the free must be ordered after it
   void* p = nullptr;
   size_t bytes = 0;
   bool owned = true;
@@ -193,6 +197,20 @@ struct Block {
 constexpr size_t kAlign = 256;
 inline size_t align_up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
 
+// Page-locked host memory of a host-resident dataset (abi_core.cpp): chunks of up to 1 GiB carved into 256-byte aligned
+// windows.  Blocks of such a dataset are ordinary Blocks whose Spans borrow windows of these chunks.  The chunks go back to
+// the context's cache when the last dataset sharing the store is freed (after every copy that may still touch them).
+struct HostStore {
+  mr_context* ctx;
+  std::vector<std::pair<void*, size_t>> chunks;
+  size_t used = 0, total = 0;  // bytes taken from the last chunk, bytes of all chunks
+  explicit HostStore(mr_context* c) : ctx(c) {}
+  ~HostStore();
+  Span take(size_t bytes);
+  HostStore(const HostStore&) = delete;
+  HostStore& operator=(const HostStore&) = delete;
+};
+
 }  // namespace mrhost
 
 namespace mrhost {
@@ -222,6 +240,7 @@ struct mr_matrix {
   std::map<std::pair<int32_t, int32_t>, mrhost::Block> blocks;
   std::shared_ptr<mrhost::ShardInfo> shard;   // set for datasets laid out on a process grid (abi_grid.cpp)
   std::vector<mrhost::Buf> temps;             // scratch that must outlive work enqueued on behalf of this dataset
+  std::shared_ptr<mrhost::HostStore> host;    // set for host-resident datasets: every block lives in this page-locked store
 };
 
 namespace mrhost {
@@ -247,8 +266,26 @@ using OutWindowFn = std::function<Span(int32_t rid, int32_t cid)>;
 // (its blocks are windows of one slab at their slots) instead of a packed one.  out_windows != nullptr (with out_layout ==
 // nullptr): every output block is written into the caller's window and the result's blocks are those windows.  The caller
 // holds ctx->mu.
+// The choices multiply_impl otherwise derives from the shape it is given.  A streamed multiply computes them once for the whole
+// product and hands them to every tile, so that each output element takes the same engine and kernel variant as in the resident
+// call: oz2 = try the Ozaki-II engine, variant = DMMA tile variant (gemm_variant still overrides it).
+struct MultiplyDecisions {
+  bool oz2 = false;
+  int variant = 0;
+};
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
-                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr);
+                         int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr,
+                         const MultiplyDecisions* decisions = nullptr);
+// The decisions multiply_impl would take for left x right, from block metadata only (the blocks may be host-resident).
+MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, const mr_matrix* right, int64_t leftColNum,
+                                     int64_t rightRowNum, int32_t blkSize);
+// Bytes of Ozaki-II residue scratch multiply_impl allocates for an nr x nc grid of output blocks (the ozaki_scratch_mb rule).
+size_t oz2_scratch_for(const mr_context* ctx, int32_t blk, int64_t K, int nr, int nc);
+// The streamed multiply (abi_stream.cpp): at least one operand is host-resident; the result is host-resident.
+mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right,
+                             int64_t rightRowNum, int64_t rightColNum, int32_t blkSize);
+// MR_ENOTSUP for a host-resident operand of an operator that only runs on device datasets.
+void require_device(const mr_matrix* m, const char* op);
 }  // namespace mrhost
 
 namespace mrhost {

@@ -93,6 +93,16 @@ class MatfastSession:
 
     toDS = createDataset
 
+    def createHostDataset(self, blocks: Iterable[MatrixBlock] = ()) -> "Dataset":
+        """A host-resident dataset: the blocks are copied into page-locked host memory owned by the engine (the arrays passed in
+        are free again at once).  ``matrixMultiply`` streams such operands through the device tile by tile, so products larger
+        than device memory run; every other operator needs :meth:`Dataset.toDevice` first."""
+        h = C.c_void_p()
+        N.check(N.lib.mr_matrix_create_host(self._ctx, C.byref(h)))
+        ds = Dataset(self, h)
+        ds.put_blocks(blocks)
+        return ds
+
     def emptyDataset(self) -> "Dataset":
         return Dataset._new(self)
 
@@ -189,7 +199,7 @@ def grid_multiply_rows(session: "MatfastSession", A_rows: "Dataset", leftRowNum:
 
 
 class Dataset:
-    """A bag of ``(rid, cid, block)`` rows resident in HBM (an ``mr_matrix`` handle)."""
+    """A bag of ``(rid, cid, block)`` rows resident in HBM, or in page-locked host memory (``isHost``) (an ``mr_matrix`` handle)."""
 
     def __init__(self, session: MatfastSession, handle: C.c_void_p):
         self.matfastSession = session
@@ -319,6 +329,22 @@ class Dataset:
     def collect(self) -> List[MatrixBlock]:
         """``.collect()`` / ``.rdd.foreach``: every row back on the host, ordered by (rid, cid)."""
         return [MatrixBlock(r, c, self.get_block(r, c)) for r, c in self.block_ids()]
+
+    # -- residence ------------------------------------------------------------------------------
+    @property
+    def isHost(self) -> bool:
+        """True when the blocks live in page-locked host memory (``createHostDataset`` / ``toHost``)."""
+        out = C.c_int32()
+        N.check(N.lib.mr_matrix_is_host(self._h, C.byref(out)))
+        return bool(out.value)
+
+    def toHost(self) -> "Dataset":
+        """A host-resident copy (ids, shapes, formats and isTransposed flags kept)."""
+        return self._unary(N.lib.mr_matrix_to_host)
+
+    def toDevice(self) -> "Dataset":
+        """A device-resident copy; the copy runs on the ingest stream and a multiply may start before it has finished."""
+        return self._unary(N.lib.mr_matrix_to_device)
 
     # -- operators: signatures of M/Dataset.scala:57-152 ----------------------------------------
     def _binary(self, fn, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize) -> "Dataset":

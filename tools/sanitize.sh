@@ -20,6 +20,7 @@ run memcheck spmm2   "spmm2_vs_oracle and (700 or 0.05 or False) or spmm2_accumu
 run memcheck sprand  "device_sprand and 512"
 run memcheck grid    "grid_multiply_matches_oracle and 1-4-1024 or sharded_put_block"
 run memcheck ksplit  "ksplit_matches_oracle and (1-1-gram or 2-1-odd or 2-4-k3 or 8-1-single)" tests/test_gpu_grid_ksplit.py  # world 1 and multi-GPU, 128-bit and scalar reduce paths
+run memcheck stream  "ragged_absent_and_transposed_blocks and 1 or sparse_times_sparse_keeps" tests/test_gpu_streamed.py  # tiled, double-buffered panels, write-back of dense and sparse C blocks
 run synccheck crt    "crt_multiply_vs_oracle and (256-256-256 or 1024)"
 run synccheck spmm2  "spmm2_vs_oracle and 700"
 run racecheck crt2sm "crt_multiply_vs_oracle and 1024"
