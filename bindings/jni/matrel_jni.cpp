@@ -155,6 +155,30 @@ MR_JNI(jlong, toDevice)(JNIEnv* env, jclass, jlong m) {
   if (throw_if(env, mr_matrix_to_device(ptr<mr_matrix>(m), &out))) return 0;
   return reinterpret_cast<jlong>(out);
 }
+// a whole matrix: `values` column-major (DenseMatrix.values of an nrows x ncols matrix), staged in pageable native memory, so it is
+// free again when mr_matrix_from_dense returns
+MR_JNI(jlong, matrixFromArray)(JNIEnv* env, jclass, jlong ctx, jdoubleArray jvalues, jlong nrows, jlong ncols, jint blkSize) {
+  if (jvalues == nullptr || nrows <= 0 || ncols <= 0 || env->GetArrayLength(jvalues) != nrows * ncols) {
+    throw_iae(env, "requirement failed: values must hold nrows * ncols elements");
+    return 0;
+  }
+  std::vector<double> values(static_cast<size_t>(nrows * ncols));
+  env->GetDoubleArrayRegion(jvalues, 0, static_cast<jsize>(values.size()), values.data());
+  if (env->ExceptionCheck()) return 0;
+  mr_matrix* m = nullptr;
+  if (throw_if(env, mr_matrix_from_dense(ptr<mr_context>(ctx), values.data(), nrows, ncols, nrows, 0, blkSize, 0, nullptr, &m))) return 0;
+  return reinterpret_cast<jlong>(m);
+}
+// DenseMatrix.toArray for the whole dataset into `out` (column-major, nrows * ncols elements, allocated by the caller)
+MR_JNI(void, matrixToArray)(JNIEnv* env, jclass, jlong m, jlong nrows, jlong ncols, jint blkSize, jdoubleArray out) {
+  if (out == nullptr || nrows <= 0 || ncols <= 0 || env->GetArrayLength(out) != nrows * ncols) {
+    throw_iae(env, "requirement failed: the destination must hold nrows * ncols elements");
+    return;
+  }
+  std::vector<double> values(static_cast<size_t>(nrows * ncols));
+  if (throw_if(env, mr_matrix_to_dense(ptr<mr_matrix>(m), nrows, ncols, blkSize, values.data(), nrows, 0, nullptr))) return;
+  env->SetDoubleArrayRegion(out, 0, static_cast<jsize>(values.size()), values.data());
+}
 MR_JNI(void, putBlock)(JNIEnv* env, jclass, jlong m, jint rid, jint cid, jbyte type, jint numRows, jint numCols, jintArray colPtrs,
                        jintArray rowIndices, jdoubleArray values, jboolean isTransposed) {
   StagedBlock b(env, type, numRows, numCols, colPtrs, rowIndices, values, isTransposed);

@@ -23,6 +23,8 @@ private[b200] object Native {
   @native def putBlock(m: Long, rid: Int, cid: Int, tpe: Byte, numRows: Int, numCols: Int,
                        colPtrs: Array[Int], rowIndices: Array[Int], values: Array[Double],
                        isTransposed: Boolean): Unit
+  @native def matrixFromArray(ctx: Long, values: Array[Double], nrows: Long, ncols: Long, blk: Int): Long
+  @native def matrixToArray(m: Long, nrows: Long, ncols: Long, blk: Int, out: Array[Double]): Unit
   @native def numBlocks(m: Long): Long
   @native def hasBlock(m: Long, rid: Int, cid: Int): Boolean
   @native def blockIds(m: Long): Array[Int] // (rid, cid) pairs, ascending
@@ -112,6 +114,11 @@ class B200Session(device: Int = -1, compatBugs: Boolean = true, gemmAlgo: Int = 
     blocks.foreach(b => Native.put(h, b, Native.putBlock))
     new B200Dataset(this, h)
   }
+
+  /** A whole nrows x ncols matrix (values column-major, as DenseMatrix.values) as a dataset of blkSize x blkSize DenseMatrix
+   *  blocks, every block present; cut on the device */
+  def fromArray(values: Array[Double], nrows: Long, ncols: Long, blkSize: Int): B200Dataset =
+    new B200Dataset(this, Native.matrixFromArray(ctx, values, nrows, ncols, blkSize))
 }
 
 class B200Dataset private[b200](val session: B200Session, private[b200] val h: Long) {
@@ -123,6 +130,13 @@ class B200Dataset private[b200](val session: B200Session, private[b200] val h: L
   def getBlock(rid: Int, cid: Int): MLMatrix =
     Native.readBlock(Native.blockMeta(h, rid, cid), (cp, ri, v) => Native.blockArrays(h, rid, cid, cp, ri, v))
   def collect(): Seq[MatrixBlock] = blockIds.map { case (i, j) => MatrixBlock(i, j, getBlock(i, j)) }
+  /** DenseMatrix.toArray (matrix/MLMatrix.scala:55-61) for the whole dataset: column-major, absent blocks are zeros */
+  def toArray(nrows: Long, ncols: Long, blkSize: Int): Array[Double] = {
+    require(nrows * ncols <= Int.MaxValue, s"a $nrows x $ncols matrix does not fit one JVM array")
+    val out = new Array[Double]((nrows * ncols).toInt)
+    Native.matrixToArray(h, nrows, ncols, blkSize, out)
+    out
+  }
 
   // ---- residence
   def isHost: Boolean = Native.isHost(h)

@@ -173,6 +173,33 @@ MR_API mr_status mr_matrix_is_host(const mr_matrix* m, int32_t* out);
 MR_API mr_status mr_matrix_to_host(mr_matrix* m, mr_matrix** out);
 MR_API mr_status mr_matrix_to_device(mr_matrix* m, mr_matrix** out);
 
+/* ---- whole dense matrices: Seq(MatrixBlock) of DenseMatrix blocks cut from one array, and DenseMatrix.toArray (M/matrix/MLMatrix.scala:55-61)
+ *      for a whole dataset.  Element (i, j) of a column-major matrix (rowMajor = 0) is at p[i + ld*j], of a row-major one
+ *      (rowMajor = 1) at p[i*ld + j]; ld must be at least the contiguous dimension (nrows, or ncols when row-major).  nrows, ncols,
+ *      blkSize > 0, and the block grid must fit Int ids (MR_EINVAL otherwise).  The host only copies; layout changes run on the GPU. */
+/* The nrows x ncols matrix at src as a dataset of blkSize x blkSize blocks (ragged at the bottom / right edge), EVERY block present.
+ * Blocks of a row-major src are stored row-major, isTransposed = 1: a row-major sub-block IS the reference's transposed dense block
+ * (M/matrix/MLMatrix.scala:285-289), so no element is transposed on the way in.  src may be host memory (pageable or page-locked)
+ * or device memory of this context's GPU (MR_EINVAL for another GPU's).  host_resident != 0: a host-resident dataset (see above).
+ * stream (cudaStream_t): the copies first wait for the work enqueued on it so far (the producer of a device src; NULL = none).
+ * Device-resident result: the copies run on the ingest stream, each block with its own event and ingest number for a host src (one
+ * gather kernel and one event for a device src), so a multiply issued right after the call starts on the blocks that have landed.
+ * WHEN src may be reused: as mr_matrix_put_block -- PAGEABLE host memory is free when the call returns; PAGE-LOCKED host memory and
+ * DEVICE memory are read asynchronously and must stay valid and unmodified until mr_matrix_wait_ingest(*out) or mr_sync(ctx) has
+ * returned.  A host-resident result from host memory is copied before the call returns. */
+MR_API mr_status mr_matrix_from_dense(mr_context* ctx, const double* src, int64_t nrows, int64_t ncols, int64_t ld, int32_t rowMajor,
+                                      int32_t blkSize, int32_t host_resident, void* stream, mr_matrix** out);
+/* The dataset as one dense nrows x ncols matrix at dst (host or device memory of this context's GPU): block (rid, cid) covers rows
+ * rid*blkSize .. and columns cid*blkSize ..; absent blocks and the part of a cell a smaller block leaves are zeros, sparse blocks (CSC
+ * or CSR) are scattered, every block's isTransposed flag is honoured.  Any residence, sharded datasets included (blocks a rank does
+ * not hold are absent).  A block outside the matrix (numRows > blkSize, rid*blkSize + numRows > nrows, or the same for columns)
+ * fails with MR_EDIM.  A host dst is filled panel by panel (block rows of a row-major dst, block columns of a column-major one)
+ * through two device buffers; their memory, and the staging of host-resident blocks, follow the option "stream_budget_mb"
+ * (MR_ENOMEM when one panel does not fit).  stream (cudaStream_t): the assembly first waits for the work enqueued on it so far, and
+ * it then waits for the assembly (the consumer of dst) -- no host wait; NULL = the call returns once dst is written. */
+MR_API mr_status mr_matrix_to_dense(mr_matrix* m, int64_t nrows, int64_t ncols, int32_t blkSize, double* dst, int64_t ld,
+                                    int32_t rowMajor, void* stream);
+
 /* ---- operators: argument-for-argument with M/Dataset.scala:57-152 and the physical operators
  *      of M/execution/MatfastExecution.scala. */
 /* Dataset.matrixMultiply :134-142 -> MatrixMatrixMultiplicationExecution :688-726 ->

@@ -63,6 +63,10 @@ class MatfastSession {
   mr_context* raw() const { return ctx_; }
   // an empty host-resident dataset (blocks in page-locked host memory); defined after Dataset
   Dataset createHostDataset();
+  // a whole nrows x ncols matrix (host or device memory, column- or row-major with leading dimension ld) as a dataset of blkSize
+  // blocks, every block present (mr_matrix_from_dense: the lifetime rule of src is put_block's); defined after Dataset
+  Dataset fromDense(const double* src, int64_t nrows, int64_t ncols, int64_t ld, bool rowMajor, int32_t blkSize,
+                    bool hostResident = false, void* stream = nullptr);
 
  private:
   mr_context* ctx_ = nullptr;
@@ -147,6 +151,17 @@ class Dataset {
     return m;
   }
 
+  // DenseMatrix.toArray for the whole dataset (mr_matrix_to_dense): absent blocks are zeros; dst in host or device memory
+  void toDense(int64_t nrows, int64_t ncols, int32_t blkSize, double* dst, int64_t ld, bool rowMajor, void* stream = nullptr) const {
+    check(mr_matrix_to_dense(h_.get(), nrows, ncols, blkSize, dst, ld, rowMajor ? 1 : 0, stream));
+  }
+  // the same as a column-major host array (DenseMatrix.values of the whole matrix)
+  std::vector<double> toDense(int64_t nrows, int64_t ncols, int32_t blkSize) const {
+    std::vector<double> out(static_cast<size_t>(nrows) * static_cast<size_t>(ncols));
+    toDense(nrows, ncols, blkSize, out.data(), nrows, false);
+    return out;
+  }
+
   // ---- operators (Dataset.scala:57-152) -----------------------------------------------------
   Dataset matrixMultiply(int64_t leftRowNum, int64_t leftColNum, const Dataset& right, int64_t rightRowNum,
                          int64_t rightColNum, int32_t blkSize) const {
@@ -228,6 +243,13 @@ class Dataset {
 inline Dataset MatfastSession::createHostDataset() {
   mr_matrix* h = nullptr;
   check(mr_matrix_create_host(ctx_, &h));
+  return Dataset(*this, h);
+}
+
+inline Dataset MatfastSession::fromDense(const double* src, int64_t nrows, int64_t ncols, int64_t ld, bool rowMajor, int32_t blkSize,
+                                         bool hostResident, void* stream) {
+  mr_matrix* h = nullptr;
+  check(mr_matrix_from_dense(ctx_, src, nrows, ncols, ld, rowMajor ? 1 : 0, blkSize, hostResident ? 1 : 0, stream, &h));
   return Dataset(*this, h);
 }
 

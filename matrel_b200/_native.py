@@ -121,6 +121,8 @@ SIGNATURES = {
     "mr_matrix_is_host": [_P, C.POINTER(_i32)],
     "mr_matrix_to_host": [_P, _PP],
     "mr_matrix_to_device": [_P, _PP],
+    "mr_matrix_from_dense": [_P, _P, _i64, _i64, _i64, _i32, _i32, _i32, _P, _PP],
+    "mr_matrix_to_dense": [_P, _i64, _i64, _i32, _P, _i64, _i32, _P],
     "mr_matrix_rand": [_P, _i64, _i64, _i32, _i64, _PP],
     "mr_matrix_sprand": [_P, _i64, _i64, _i32, _f64, _i64, C.c_uint8, _PP],
     "mr_matrix_rand_partition": [_P, _i64, _i64, _i32, _i64, _i32, _i32, _i32, _i32, _P, _i64, _PP],

@@ -17,6 +17,22 @@ using namespace mrhost;
 
 namespace mrhost {
 
+size_t stream_budget(mr_context* ctx, size_t enough) {
+  if (ctx->stream_budget_mb > 0) return static_cast<size_t>(ctx->stream_budget_mb) << 20;
+  size_t free_b = 0, total_b = 0;
+  if (enough != SIZE_MAX) {  // the pool's cache stays when the memory free without it is enough
+    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    if (free_b > (1ull << 30) && free_b - (1ull << 30) >= enough) return free_b - (1ull << 30);
+  }
+  // free memory at the call, with what this device's pool caches handed back first, minus 1 GiB of headroom
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  cudaMemPool_t pool;
+  if (cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);
+  (void)cudaGetLastError();
+  CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+  return free_b > (1ull << 30) ? free_b - (1ull << 30) : 0;
+}
+
 // The tiling rule.  Inputs: nr block rows of A and nc block columns of B take part; a_row / b_col = device bytes of the largest
 // block row of A / block column of B when that operand is host-resident (0 when it is used in place); a_bytes / b_bytes = its
 // host -> device payload (0 in place); c_block = device bytes of the largest output block; scratch(tr, tc) = what a tr x tc tile
@@ -140,18 +156,7 @@ mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNu
   const size_t a_scratch = a_sparse ? a_row_dense + a_row_fp : 0;
   const size_t b_scratch = ((b_sparse ? 1 : 0) + (a_sparse ? 1 : 0)) * b_col_dense;
   // ---- device budget and the tile
-  size_t budget;
-  if (ctx->stream_budget_mb > 0) {
-    budget = static_cast<size_t>(ctx->stream_budget_mb) << 20;
-  } else {  // free memory at the call, with what this device's pool caches handed back first, minus 1 GiB of headroom
-    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);
-    (void)cudaGetLastError();
-    size_t free_b = 0, total_b = 0;
-    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-    budget = free_b > (1ull << 30) ? free_b - (1ull << 30) : 0;
-  }
+  const size_t budget = stream_budget(ctx);
   const size_t c_block = align_up(static_cast<size_t>(max_m) * max_n * sizeof(double));
   const StreamTiling T = choose_tiling(
       static_cast<int64_t>(rows.size()), static_cast<int64_t>(cols.size()), a_row, b_col, a_bytes, b_bytes, c_block, budget,

@@ -284,6 +284,10 @@ size_t oz2_scratch_for(const mr_context* ctx, int32_t blk, int64_t K, int nr, in
 // The streamed multiply (abi_stream.cpp): at least one operand is host-resident; the result is host-resident.
 mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right,
                              int64_t rightRowNum, int64_t rightColNum, int32_t blkSize);
+// Device memory a streamed multiply or a panelled mr_matrix_to_dense may use (abi_stream.cpp): the option stream_budget_mb, or
+// when it is 0 the free device memory at the call minus 1 GiB, counted after the device's memory pool has handed its cache back
+// (a synchronisation of the context stream) unless the memory free without that is already `enough`.
+size_t stream_budget(mr_context* ctx, size_t enough = SIZE_MAX);
 // MR_ENOTSUP for a host-resident operand of an operator that only runs on device datasets.
 void require_device(const mr_matrix* m, const char* op);
 }  // namespace mrhost

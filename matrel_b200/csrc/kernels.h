@@ -293,6 +293,33 @@ constexpr int kKsplitMaxParts = 64;
 cudaError_t launch_ksplit_reduce(const KsplitDesc* d_descs, int ndescs, const double* const* d_parts, int nparts, int64_t max_count,
                                  cudaStream_t stream);
 
+// Whole dense matrices <-> blocks (dense_io.cu, abi_dense.cpp).  A window: rows x cols logical elements; a row-major side (rm = 1)
+// holds element (r, c) at p[r * ld + c], a column-major one at p[r + c * ld].
+struct DenseIoDesc {
+  const double* src;      // nullptr (assemble only): the window is zero-filled
+  double* dst;
+  int64_t lds, ldd;       // leading dimensions, elements
+  int32_t rows, cols;
+  uint8_t src_rm, dst_rm;
+  uint8_t pad[6];
+};
+// gather: src and dst share one layout (src_rm == dst_rm); assemble: any pair of layouts (any_transposed: some src_rm != dst_rm)
+cudaError_t launch_dense_gather(const DenseIoDesc* d_descs, int ndescs, int max_rows, int max_cols, cudaStream_t stream);
+cudaError_t launch_dense_assemble(const DenseIoDesc* d_descs, int ndescs, int max_rows, int max_cols, bool any_transposed,
+                                  cudaStream_t stream);
+// The entries of a CSC (csr = 0) or CSR (csr = 1) block into its window of dst, after that window was zero-filled.
+struct DenseScatterDesc {
+  const int32_t* ptrs;    // nlines + 1
+  const int32_t* idx;
+  const double* vals;
+  double* dst;            // the window's element (0, 0)
+  int64_t ldd;
+  int32_t nlines;         // columns (CSC) or rows (CSR)
+  uint8_t csr, dst_rm;
+  uint8_t pad[2];
+};
+cudaError_t launch_dense_scatter(const DenseScatterDesc* d_descs, int ndescs, int max_lines, cudaStream_t stream);
+
 // java.util.Random-compatible U(0,1) fill: out[i] = i-th nextDouble() of new Random(seed), batched over blocks
 struct RandDesc {
   double* out;

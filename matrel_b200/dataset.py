@@ -38,6 +38,7 @@ class MatfastSession:
                             C.c_void_p(stream) if stream else None)
         self._ctx = C.c_void_p()
         N.check(N.lib.mr_init(C.byref(opts), C.byref(self._ctx)))
+        self._device = int(device)
 
     # -- lifetime ---------------------------------------------------------------------------
     def stop(self) -> None:
@@ -106,12 +107,75 @@ class MatfastSession:
     def emptyDataset(self) -> "Dataset":
         return Dataset._new(self)
 
+    def _cuda_device(self) -> int:
+        if self._device >= 0:
+            return self._device
+        import torch
+        return torch.cuda.current_device()
+
+    def fromDense(self, a, blkSize: int, host: bool = False) -> "Dataset":
+        """A whole 2-D float64 matrix as a dataset of ``blkSize`` blocks, every block present (``mr_matrix_from_dense``).  ``a`` is a
+        numpy array or a torch tensor with one unit-stride dimension (C order, F order, or a slice of either); blocks of a row-major
+        ``a`` are stored row-major (``isTransposed``), so nothing is transposed on the way in.  A CUDA tensor must be on the session's
+        device; its copy is ordered after ``torch.cuda.current_stream()``.  ``host``: a host-resident dataset.  A CUDA tensor or a
+        page-locked CPU tensor is read asynchronously: the dataset keeps a reference to it, and it must not be modified before
+        :meth:`Dataset.wait_ingest` (or :meth:`sync`)."""
+        keep, stream = None, None
+        if not isinstance(a, np.ndarray):
+            import torch
+            if not isinstance(a, torch.Tensor):
+                raise TypeError(f"fromDense takes a numpy array or a torch tensor, got {type(a).__name__}")
+            if a.dtype != torch.float64:
+                raise TypeError(f"fromDense needs float64 data, got a tensor of {a.dtype}")
+            if a.device.type == "cuda":
+                if a.device.index != self._cuda_device():
+                    raise ValueError(f"fromDense: the tensor is on {a.device}, the session runs on cuda:{self._cuda_device()}")
+                keep, stream = a, _torch_stream(a.device)
+                ptr, shape, strides = a.data_ptr(), tuple(a.shape), tuple(a.stride())
+            elif a.device.type == "cpu":
+                if a.is_pinned():
+                    keep = a
+                a = a.detach().numpy()
+            else:
+                raise ValueError(f"fromDense: a tensor on device {a.device} (CPU and CUDA tensors only)")
+        if isinstance(a, np.ndarray):
+            if a.dtype != np.float64:
+                raise TypeError(f"fromDense needs float64 data, got an array of {a.dtype}")
+            ptr, shape, strides = a.ctypes.data, a.shape, tuple(s // a.itemsize if s % a.itemsize == 0 else 0 for s in a.strides)
+        if len(shape) != 2:
+            raise ValueError(f"fromDense needs a 2-D matrix, got shape {shape}")
+        rowMajor, ld = _dense_layout(shape, strides)
+        h = C.c_void_p()
+        N.check(N.lib.mr_matrix_from_dense(self._ctx, C.c_void_p(ptr), shape[0], shape[1], ld, rowMajor, int(blkSize),
+                                           1 if host else 0, C.c_void_p(stream) if stream else None, C.byref(h)))
+        ds = Dataset(self, h)
+        ds._source = keep
+        return ds
+
     def rand(self, nrows: int, ncols: int, blkSize: int, seed0: int) -> "Dataset":
         """Every block ``DenseMatrix.rand(r, c, new java.util.Random(seed0 + rid*nbc + cid))``
         (M/matrix/MLMatrix.scala:453-457), generated on the device."""
         h = C.c_void_p()
         N.check(N.lib.mr_matrix_rand(self._ctx, nrows, ncols, blkSize, seed0, C.byref(h)))
         return Dataset(self, h)
+
+
+def _torch_stream(device) -> int:
+    """torch's current stream on `device` as a cudaStream_t; its default stream is the legacy one (handle 0), passed as
+    cudaStreamLegacy (0x1) because NULL means "no stream" to mr_matrix_from_dense / mr_matrix_to_dense."""
+    import torch
+    return torch.cuda.current_stream(device).cuda_stream or 1
+
+
+def _dense_layout(shape, strides):
+    """(rowMajor, ld) of a 2-D matrix with element strides `strides`; the stride of a dimension of extent 1 does not matter."""
+    (r, c), (s0, s1) = shape, strides
+    if s1 == 1 and (r == 1 or s0 >= c):
+        return 1, (s0 if r > 1 else c)
+    if s0 == 1 and (c == 1 or s1 >= r):
+        return 0, (s1 if c > 1 else r)
+    raise ValueError(f"fromDense needs one unit-stride dimension (C order, F order or a slice of either); "
+                     f"got shape {tuple(shape)} with element strides {tuple(strides)}")
 
 
 def sprand(session: "MatfastSession", nrows: int, ncols: int, blkSize: int, density: float, seed0: int, csr: bool = True) -> "Dataset":
@@ -329,6 +393,27 @@ class Dataset:
     def collect(self) -> List[MatrixBlock]:
         """``.collect()`` / ``.rdd.foreach``: every row back on the host, ordered by (rid, cid)."""
         return [MatrixBlock(r, c, self.get_block(r, c)) for r, c in self.block_ids()]
+
+    def toNumpy(self, nrows: int, ncols: int, blkSize: int, order: str = "C") -> np.ndarray:
+        """The dataset as one ``nrows x ncols`` array (``mr_matrix_to_dense``): absent blocks are zeros, sparse blocks scattered,
+        ``isTransposed`` honoured; assembled on the device, panel by panel."""
+        if order not in ("C", "F"):
+            raise ValueError(f"order must be 'C' or 'F', got {order!r}")
+        out = np.empty((int(nrows), int(ncols)), dtype=np.float64, order=order)
+        rowMajor = 1 if order == "C" else 0
+        N.check(N.lib.mr_matrix_to_dense(self._h, int(nrows), int(ncols), int(blkSize), C.c_void_p(out.ctypes.data),
+                                         int(ncols) if rowMajor else int(nrows), rowMajor, None))
+        return out
+
+    def toTorch(self, nrows: int, ncols: int, blkSize: int):
+        """The same as a contiguous float64 CUDA tensor on the session's device; ``torch.cuda.current_stream()`` is ordered behind
+        the assembly (no host wait)."""
+        import torch
+        dev = torch.device("cuda", self.matfastSession._cuda_device())
+        out = torch.empty((int(nrows), int(ncols)), dtype=torch.float64, device=dev)
+        N.check(N.lib.mr_matrix_to_dense(self._h, int(nrows), int(ncols), int(blkSize), C.c_void_p(out.data_ptr()), int(ncols), 1,
+                                         C.c_void_p(_torch_stream(dev))))
+        return out
 
     # -- residence ------------------------------------------------------------------------------
     @property
