@@ -399,6 +399,9 @@ typedef struct mr_stats {
   int64_t stream_tiles;     /* C tiles of the most recent streamed multiply (a host-resident operand; mr_matrix_create_host) */
   int64_t stream_h2d_bytes; /* operand panels that multiply moved host -> device (h2d_bytes also counts its descriptor tables) */
   int64_t stream_d2h_bytes; /* result blocks that multiply moved device -> host */
+  int64_t spgemm_pairs;     /* block pairs of the most recent mr_matrix_multiply computed by the sparse x sparse kernel (output blocks
+                               whose partials are all low-density sparse x sparse; summed over the tiles of a streamed multiply) */
+  int64_t spgemm_products;  /* scalar products that kernel performed: sum over its pairs and k of nnz(A(:,k)) * nnz(B(k,:)) */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

@@ -75,6 +75,8 @@ class mr_stats(C.Structure):
         ("stream_tiles", C.c_int64),
         ("stream_h2d_bytes", C.c_int64),
         ("stream_d2h_bytes", C.c_int64),
+        ("spgemm_pairs", C.c_int64),
+        ("spgemm_products", C.c_int64),
     ]
 
 

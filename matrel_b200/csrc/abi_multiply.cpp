@@ -497,133 +497,291 @@ struct Oz2Run {
 
 // ------------------------------------------------------------------------------------------------
 // Output blocks whose partial products are ALL low-density sparse x sparse (LocalMatrix.multiplySparseSparse,
-// LocalMatrix.scala:143-323).  Values: each partial is computed as sparse A x densified B (the same sums in a different
-// order).  Storage format: the reference's four loop nests end in four different rules, and `reduceByKey(LocalMatrix.add)`
-// re-decides the format at every sparse + sparse step, so the chain is replayed partial by partial in ascending k (Spark's
-// own reduce order is arbitrary; ascending k is the deterministic choice):
+// LocalMatrix.scala:143-323), computed natively on the stored entries by spgemm.cu.  Storage format: the reference's four loop
+// nests end in four different rules, and `reduceByKey(LocalMatrix.add)` re-decides the format at every sparse + sparse step, so
+// the chain is replayed partial by partial in ascending k (Spark's own reduce order is arbitrary; ascending k is the
+// deterministic choice):
 //   CSC x CSC (:155-196): CSC iff rows*cols > 2 nnz + cols + 1, else dense      CSR x CSR (:198-239): CSR iff ... + rows + 1
 //   CSR x CSC (:241-286): always CSC (both branches build a SparseMatrix)       CSC x CSR (:288-323): dense iff rows*cols <= 2 nnz + cols
 //   sparse + sparse (:74-139): CSC iff rows*cols > 2 nnz + cols + 1, else dense; anything + dense: dense.
+// The values do not depend on these formats (every product and sum is rounded on its own and zeros are dropped after each, so a
+// dense partial sum holds exactly the sparse one's entries), so the device computes every chain sparsely and the rules only need
+// nnz(P_l) and nnz(S_l) of each level: a count pass returns them in ONE read-back, the host replays the rules, and a fill pass
+// writes each result in its final format (a dense window only for chains that end dense).
 // ------------------------------------------------------------------------------------------------
 enum ChainFmt { FMT_DENSE = 0, FMT_CSC = 1, FMT_CSR = 2 };
 
-void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<size_t>& chains,
-                       const std::vector<double*>& cptr, MultiplyPlanner& planner, mr_matrix* result) {
+int partial_format(bool aT, bool bT, int64_t m, int64_t n, int64_t nnz) {
+  const int64_t cells = m * n;
+  if (!aT && !bT) return cells > 2 * nnz + n + 1 ? FMT_CSC : FMT_DENSE;
+  if (aT && bT) return cells > 2 * nnz + m + 1 ? FMT_CSR : FMT_DENSE;
+  if (aT && !bT) return FMT_CSC;
+  return cells <= 2 * nnz + n ? FMT_DENSE : FMT_CSC;
+}
+
+void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<size_t>& chains_all,
+                       const std::vector<double*>& cptr, mr_matrix* result) {
+  std::vector<size_t> chains;  // empty output blocks keep the (empty) dense block run_multiply gave them
+  for (size_t i : chains_all)
+    if (plans[i].m > 0 && plans[i].n > 0) chains.push_back(i);
   if (chains.empty()) return;
-  size_t levels = 0;
-  for (size_t i : chains) levels = std::max(levels, plans[i].spsp.size());
-  std::vector<int> fmt(chains.size(), FMT_DENSE);
-  std::vector<Buf> scratch(chains.size());
-  for (size_t lv = 0; lv < levels; ++lv) {
-    std::vector<size_t> act;  // chains that have a partial at this level
-    std::vector<DenseWin> pw;
-    for (size_t c = 0; c < chains.size(); ++c) {
-      OutPlan& o = plans[chains[c]];
-      if (lv >= o.spsp.size() || o.m == 0 || o.n == 0) continue;
-      const Block& a = *o.spsp[lv].first;
-      const Block& b = planner.dense_of(*o.spsp[lv].second);
-      wait_ready(ctx, a);
-      wait_ready(ctx, *o.spsp[lv].second);
-      const size_t bytes = static_cast<size_t>(o.m) * o.n * sizeof(double);
-      double* target = cptr[chains[c]];
-      if (lv > 0) {
-        if (!scratch[c]) scratch[c] = std::make_shared<DevBuf>(ctx, bytes);
-        target = static_cast<double*>(scratch[c]->p);
+  const size_t nc = chains.size();
+  // ---- frames: an all-CSR chain runs as C^T = B^T A^T on the CSR arrays; any other chain in CSC, its CSR operands converted once
+  std::vector<char> csr_frame(nc, 1);
+  for (size_t c = 0; c < nc; ++c)
+    for (auto& pr : plans[chains[c]].spsp) {
+      wait_ready(ctx, *pr.first);
+      wait_ready(ctx, *pr.second);
+      if (!pr.first->isT || !pr.second->isT) csr_frame[c] = 0;
+    }
+  struct Conv {
+    size_t ptr, idx, val, cur;  // byte offsets in the conversion buffer
+  };
+  std::map<const Block*, Conv> conv;
+  size_t conv_bytes = 0;
+  auto need_conv = [&](const Block* b) {
+    if (!b->isT || conv.count(b)) return;
+    Conv v;
+    v.ptr = conv_bytes;
+    conv_bytes += align_up(static_cast<size_t>(b->numCols + 1) * sizeof(int32_t));
+    v.idx = conv_bytes;
+    conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(int32_t));
+    v.val = conv_bytes;
+    conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(double));
+    v.cur = conv_bytes;
+    conv_bytes += align_up(static_cast<size_t>(b->numCols) * sizeof(int32_t));
+    conv.emplace(b, v);
+  };
+  for (size_t c = 0; c < nc; ++c)
+    if (!csr_frame[c])
+      for (auto& pr : plans[chains[c]].spsp) {
+        need_conv(pr.first);
+        need_conv(pr.second);
       }
-      if (!a.isT) CUDA_CHECK(cudaMemsetAsync(target, 0, bytes, ctx->stream));  // the CSC kernel scatters into zeros
-      CUDA_CHECK(launch_spmm(a.colPtrs.ptr<int32_t>(), a.rowIndices.ptr<int32_t>(), a.values.ptr<double>(), a.isT,
-                             b.values.ptr<double>(), b.isT, target, a.numRows, a.numCols, b.numCols, false, ctx->stream));
-      note_launch(ctx);
-      act.push_back(c);
-      pw.push_back(DenseWin{target, o.m, o.n});
+  Buf cbuf;
+  if (!conv.empty()) {
+    cbuf = std::make_shared<DevBuf>(ctx, conv_bytes);
+    CUDA_CHECK(cudaMemsetAsync(cbuf->p, 0, conv_bytes, ctx->stream));
+    char* base = static_cast<char*>(cbuf->p);
+    std::vector<SpTransDesc> td;
+    std::vector<ScanDesc> sd;
+    int max_nnz = 0, max_nl = 0, max_no = 0;
+    for (auto& kv : conv) {
+      const Block* b = kv.first;
+      const Conv& v = kv.second;
+      SpTransDesc d{};
+      d.ptr = b->colPtrs.ptr<int32_t>();
+      d.idx = b->rowIndices.ptr<int32_t>();
+      d.val = b->values.ptr<double>();
+      d.nl = b->numRows;
+      d.no = b->numCols;
+      d.nnz = static_cast<int32_t>(b->valuesLen);
+      d.optr = reinterpret_cast<int32_t*>(base + v.ptr);
+      d.oidx = reinterpret_cast<int32_t*>(base + v.idx);
+      d.oval = reinterpret_cast<double*>(base + v.val);
+      d.cur = reinterpret_cast<int32_t*>(base + v.cur);
+      td.push_back(d);
+      sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
+      max_nnz = std::max(max_nnz, d.nnz);
+      max_nl = std::max(max_nl, d.nl);
+      max_no = std::max(max_no, d.no);
     }
-    if (act.empty()) continue;
-    const auto pcounts = column_counts(ctx, pw);
-    std::vector<size_t> recount;  // chains whose running sum is sparse + sparse at this level
-    std::vector<EwDesc> adds;
-    int max_rows = 0, max_cols = 0;
-    for (size_t t = 0; t < act.size(); ++t) {
-      const size_t c = act[t];
-      OutPlan& o = plans[chains[c]];
-      const bool aT = o.spsp[lv].first->isT, bT = o.spsp[lv].second->isT;
-      const int64_t cells = static_cast<int64_t>(o.m) * o.n, nnz = total_count(pcounts[t]);
-      int pf;
-      if (!aT && !bT) pf = cells > 2 * nnz + o.n + 1 ? FMT_CSC : FMT_DENSE;
-      else if (aT && bT) pf = cells > 2 * nnz + o.m + 1 ? FMT_CSR : FMT_DENSE;
-      else if (aT && !bT) pf = FMT_CSC;
-      else pf = cells <= 2 * nnz + o.n ? FMT_DENSE : FMT_CSC;
-      if (lv == 0) {
-        fmt[c] = pf;
-        continue;
-      }
-      EwDesc d{};
-      d.A = cptr[chains[c]];
-      d.B = pw[t].p;
-      d.C = cptr[chains[c]];  // in place: every element is read and written by the same thread
-      d.rows = o.m;
-      d.cols = o.n;
-      adds.push_back(d);
-      max_rows = std::max(max_rows, o.m);
-      max_cols = std::max(max_cols, o.n);
-      if (fmt[c] == FMT_DENSE || pf == FMT_DENSE) fmt[c] = FMT_DENSE;
-      else recount.push_back(c);
-    }
-    if (!adds.empty()) {
-      Buf d = upload(ctx, adds);
-      CUDA_CHECK(launch_ew_batched(EW_ADD, static_cast<const EwDesc*>(d->p), static_cast<int>(adds.size()), max_rows, max_cols,
-                                   false, ctx->stream));
-      note_launch(ctx);
-    }
-    if (!recount.empty()) {
-      std::vector<DenseWin> sw;
-      for (size_t c : recount) sw.push_back(DenseWin{cptr[chains[c]], plans[chains[c]].m, plans[chains[c]].n});
-      const auto scounts = column_counts(ctx, sw);
-      for (size_t t = 0; t < recount.size(); ++t) {
-        const OutPlan& o = plans[chains[recount[t]]];
-        fmt[recount[t]] = static_cast<int64_t>(o.m) * o.n > 2 * total_count(scounts[t]) + o.n + 1 ? FMT_CSC : FMT_DENSE;
-      }
-    }
+    Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
+    CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
+                              max_nnz, max_nl, max_no, ctx->stream));
+    note_launch(ctx, 4);
   }
-  // final storage: dense results stay in their slab window; CSC / CSR results are compacted out of it
-  std::vector<DenseWin> cw;
-  std::vector<size_t> cw_chain;
-  std::vector<Buf> keep;
-  for (size_t c = 0; c < chains.size(); ++c) {
+  // ---- the chains and their pairs in the frame
+  std::vector<SpgemmChain> ch(nc);
+  std::vector<SpgemmPair> pairs;
+  std::vector<SpgemmItem> items;
+  const int per_item = spgemm_columns_per_item();
+  int32_t count_total = 0;
+  int64_t col_total = 0;
+  int max_m = 0, max_levels = 0;
+  for (size_t c = 0; c < nc; ++c) {
     const OutPlan& o = plans[chains[c]];
-    if (o.m == 0 || o.n == 0 || fmt[c] == FMT_DENSE) continue;
-    if (fmt[c] == FMT_CSC) {
-      cw.push_back(DenseWin{cptr[chains[c]], o.m, o.n});
-    } else {  // CSR of C = CSC of C^T: materialise the row-major copy (= column-major n x m) first
-      Buf t = std::make_shared<DevBuf>(ctx, static_cast<size_t>(o.m) * o.n * sizeof(double));
-      EwDesc d{};
-      d.A = cptr[chains[c]];
-      d.C = static_cast<double*>(t->p);
-      d.rows = o.n;
-      d.cols = o.m;
-      d.aT = 1;
-      std::vector<EwDesc> one{d};
-      Buf dd = upload(ctx, one);
-      CUDA_CHECK(launch_ew_batched(EW_COPY, static_cast<const EwDesc*>(dd->p), 1, o.n, o.m, true, ctx->stream));
-      note_launch(ctx);
-      cw.push_back(DenseWin{static_cast<const double*>(t->p), o.n, o.m});
-      keep.push_back(t);
-    }
-    cw_chain.push_back(c);
-  }
-  if (!cw.empty()) {
-    const auto counts = column_counts(ctx, cw);
-    std::vector<Block> blocks = compact_csc(ctx, cw, counts);
-    for (size_t t = 0; t < blocks.size(); ++t) {
-      const size_t c = cw_chain[t];
-      const OutPlan& o = plans[chains[c]];
-      Block& b = blocks[t];
-      if (fmt[c] == FMT_CSR) {  // the CSC arrays of C^T are the CSR arrays of C
-        b.numRows = o.m;
-        b.numCols = o.n;
-        b.isT = true;
+    SpgemmChain& h = ch[c];
+    h.m = csr_frame[c] ? o.n : o.m;
+    h.n = csr_frame[c] ? o.m : o.n;
+    h.pair_begin = static_cast<int32_t>(pairs.size());
+    h.levels = static_cast<int32_t>(o.spsp.size());
+    h.count_off = count_total;
+    count_total += 2 * h.levels;
+    col_total += h.n;
+    max_m = std::max(max_m, h.m);
+    max_levels = std::max(max_levels, h.levels);
+    auto csc_of = [&](const Block* b, const int32_t*& p, const int32_t*& i, const double*& v) {
+      if (b->isT && !csr_frame[c]) {
+        const Conv& cv = conv.at(b);
+        char* base = static_cast<char*>(cbuf->p);
+        p = reinterpret_cast<const int32_t*>(base + cv.ptr);
+        i = reinterpret_cast<const int32_t*>(base + cv.idx);
+        v = reinterpret_cast<const double*>(base + cv.val);
+      } else {  // CSC, or (CSR frame) the CSC arrays of the block's transpose
+        p = b->colPtrs.ptr<int32_t>();
+        i = b->rowIndices.ptr<int32_t>();
+        v = b->values.ptr<double>();
       }
-      result->blocks[{o.rid, o.cid}] = std::move(b);
+    };
+    for (auto& pr : o.spsp) {
+      SpgemmPair q{};
+      const Block* lb = csr_frame[c] ? pr.second : pr.first;
+      const Block* rb = csr_frame[c] ? pr.first : pr.second;
+      csc_of(lb, q.lp, q.li, q.lv);
+      csc_of(rb, q.rp, q.ri, q.rv);
+      pairs.push_back(q);
     }
+    for (int32_t c0 = 0; c0 < h.n; c0 += per_item) items.push_back(SpgemmItem{static_cast<int32_t>(c), c0});
+  }
+  // ---- count pass: per-level counters, scalar products, per-column counts of the final sums
+  const size_t counts_off = 0, prod_off = align_up(static_cast<size_t>(count_total) * sizeof(int32_t)),
+               colcnt_off = prod_off + align_up(sizeof(unsigned long long));
+  Buf meta = std::make_shared<DevBuf>(ctx, colcnt_off + static_cast<size_t>(col_total) * sizeof(int32_t));
+  CUDA_CHECK(cudaMemsetAsync(meta->p, 0, colcnt_off, ctx->stream));
+  char* mbase = static_cast<char*>(meta->p);
+  int32_t* d_counts = reinterpret_cast<int32_t*>(mbase + counts_off);
+  auto* d_products = reinterpret_cast<unsigned long long*>(mbase + prod_off);
+  {
+    int64_t off = 0;
+    for (size_t c = 0; c < nc; ++c) {
+      ch[c].colcnt = reinterpret_cast<int32_t*>(mbase + colcnt_off) + off;
+      off += ch[c].n;
+    }
+  }
+  const SpgemmLaunchShape shape = spgemm_shape(max_m, max_levels);
+  Buf scratch = shape.scratch_bytes ? std::make_shared<DevBuf>(ctx, shape.scratch_bytes) : nullptr;
+  Buf d_pairs = upload(ctx, pairs), d_items = upload(ctx, items), d_ch = upload(ctx, ch);
+  CUDA_CHECK(launch_spgemm(false, static_cast<const SpgemmItem*>(d_items->p), static_cast<int>(items.size()),
+                           static_cast<const SpgemmChain*>(d_ch->p), static_cast<const SpgemmPair*>(d_pairs->p), d_counts, d_products,
+                           scratch ? scratch->p : nullptr, max_m, shape, ctx->stream));
+  note_launch(ctx);
+  std::vector<int32_t> h_counts(static_cast<size_t>(count_total));
+  unsigned long long h_products = 0;
+  CUDA_CHECK(cudaMemcpyAsync(h_counts.data(), d_counts, h_counts.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_CHECK(cudaMemcpyAsync(&h_products, d_products, sizeof(h_products), cudaMemcpyDeviceToHost, ctx->stream));
+  ctx->stats.d2h_bytes += static_cast<int64_t>(h_counts.size() * sizeof(int32_t) + sizeof(h_products));
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ctx->stats.spgemm_pairs += static_cast<int64_t>(pairs.size());
+  ctx->stats.spgemm_products += static_cast<int64_t>(h_products);
+  // ---- the reference's format rules, level by level
+  std::vector<int> fmt(nc);
+  std::vector<int64_t> nnz(nc);
+  for (size_t c = 0; c < nc; ++c) {
+    const OutPlan& o = plans[chains[c]];
+    const int32_t* cp = h_counts.data() + ch[c].count_off;
+    const int32_t* cs = cp + ch[c].levels;
+    int64_t s_nnz = 0;
+    for (int32_t l = 0; l < ch[c].levels; ++l) {
+      s_nnz += cs[l];
+      const int pf = partial_format(o.spsp[l].first->isT, o.spsp[l].second->isT, o.m, o.n, cp[l]);
+      if (l == 0) fmt[c] = pf;
+      else if (fmt[c] == FMT_DENSE || pf == FMT_DENSE) fmt[c] = FMT_DENSE;
+      else fmt[c] = static_cast<int64_t>(o.m) * o.n > 2 * s_nnz + o.n + 1 ? FMT_CSC : FMT_DENSE;
+    }
+    nnz[c] = s_nnz;
+  }
+  // ---- outputs: a dense window (the caller's, or from a slab of the dense-ending chains), or exactly sized sparse arrays
+  size_t dense_total = 0, sparse_total = 0;
+  for (size_t c = 0; c < nc; ++c) {
+    const OutPlan& o = plans[chains[c]];
+    if (fmt[c] == FMT_DENSE) {
+      if (!cptr[chains[c]]) dense_total += align_up(static_cast<size_t>(o.m) * o.n * sizeof(double));
+    } else {
+      const bool via_csr = csr_frame[c] && fmt[c] == FMT_CSC;  // S in the CSR frame, converted to CSC at the end
+      const size_t e = static_cast<size_t>(nnz[c]);
+      sparse_total += align_up((static_cast<size_t>(ch[c].n) + 1) * sizeof(int32_t)) + align_up(e * sizeof(int32_t)) +
+                      align_up(e * sizeof(double));
+      if (via_csr)
+        sparse_total += 2 * align_up((static_cast<size_t>(o.n) + 1) * sizeof(int32_t)) + align_up(e * sizeof(int32_t)) +
+                        align_up(e * sizeof(double));
+    }
+  }
+  std::unique_ptr<Slab> dslab, sslab;
+  if (dense_total) dslab.reset(new Slab(ctx, dense_total));
+  if (sparse_total) sslab.reset(new Slab(ctx, sparse_total));
+  std::vector<ScanDesc> scans;
+  std::vector<SpTransDesc> finals;
+  std::vector<ScanDesc> final_scans;
+  int fmax_nnz = 0, fmax_nl = 0, fmax_no = 0;
+  for (size_t c = 0; c < nc; ++c) {
+    const OutPlan& o = plans[chains[c]];
+    SpgemmChain& h = ch[c];
+    Block& out = result->blocks[{o.rid, o.cid}];
+    if (fmt[c] == FMT_DENSE) {
+      if (cptr[chains[c]]) {
+        h.dense = cptr[chains[c]];
+      } else {
+        Span s = dslab->take(static_cast<size_t>(o.m) * o.n * sizeof(double));
+        h.dense = s.ptr<double>();
+        out = dense_block(o.m, o.n, s, false);
+      }
+      h.drs = csr_frame[c] ? o.m : 1;
+      h.dcs = csr_frame[c] ? 1 : o.m;
+      continue;
+    }
+    const size_t e = static_cast<size_t>(nnz[c]);
+    Span ptr = sslab->take((static_cast<size_t>(h.n) + 1) * sizeof(int32_t)), idx = sslab->take(e * sizeof(int32_t)),
+         val = sslab->take(e * sizeof(double));
+    h.optr = ptr.ptr<int32_t>();
+    h.oidx = idx.ptr<int32_t>();
+    h.oval = val.ptr<double>();
+    scans.push_back(ScanDesc{h.colcnt, ptr.ptr<int32_t>(), h.n, 0});
+    Block b;
+    b.type = 0;
+    b.numRows = o.m;
+    b.numCols = o.n;
+    b.valuesLen = static_cast<int64_t>(e);
+    if (csr_frame[c] && fmt[c] == FMT_CSC) {  // CSR arrays of C -> CSC
+      Span cptr2 = sslab->take((static_cast<size_t>(o.n) + 1) * sizeof(int32_t)), cidx = sslab->take(e * sizeof(int32_t)),
+           cval = sslab->take(e * sizeof(double)), cur = sslab->take(static_cast<size_t>(o.n) * sizeof(int32_t));
+      SpTransDesc d{};
+      d.ptr = ptr.ptr<int32_t>();
+      d.idx = idx.ptr<int32_t>();
+      d.val = val.ptr<double>();
+      d.nl = o.m;
+      d.no = o.n;
+      d.nnz = static_cast<int32_t>(e);
+      d.optr = cptr2.ptr<int32_t>();
+      d.oidx = cidx.ptr<int32_t>();
+      d.oval = cval.ptr<double>();
+      d.cur = cur.ptr<int32_t>();
+      finals.push_back(d);
+      final_scans.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
+      fmax_nnz = std::max(fmax_nnz, d.nnz);
+      fmax_nl = std::max(fmax_nl, d.nl);
+      fmax_no = std::max(fmax_no, d.no);
+      CUDA_CHECK(cudaMemsetAsync(d.cur, 0, static_cast<size_t>(o.n) * sizeof(int32_t), ctx->stream));
+      b.colPtrs = cptr2;
+      b.rowIndices = cidx;
+      b.values = cval;
+      b.colPtrsLen = o.n + 1;
+      b.isT = false;
+    } else {  // the frame's arrays are the result's: CSC (CSC frame) or CSR (CSR frame)
+      b.colPtrs = ptr;
+      b.rowIndices = idx;
+      b.values = val;
+      b.colPtrsLen = h.n + 1;
+      b.isT = csr_frame[c] != 0;
+    }
+    out = std::move(b);
+  }
+  // ---- fill pass
+  if (!scans.empty()) {
+    Buf d_scans = upload(ctx, scans);
+    CUDA_CHECK(launch_exclusive_scan(static_cast<const ScanDesc*>(d_scans->p), static_cast<int>(scans.size()), ctx->stream));
+    note_launch(ctx);
+  }
+  Buf d_ch2 = upload(ctx, ch);
+  CUDA_CHECK(launch_spgemm(true, static_cast<const SpgemmItem*>(d_items->p), static_cast<int>(items.size()),
+                           static_cast<const SpgemmChain*>(d_ch2->p), static_cast<const SpgemmPair*>(d_pairs->p), d_counts, d_products,
+                           scratch ? scratch->p : nullptr, max_m, shape, ctx->stream));
+  note_launch(ctx);
+  if (!finals.empty()) {
+    Buf d_f = upload(ctx, finals), d_fs = upload(ctx, final_scans);
+    CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_f->p), static_cast<const ScanDesc*>(d_fs->p), static_cast<int>(finals.size()),
+                              fmax_nnz, fmax_nl, fmax_no, ctx->stream));
+    note_launch(ctx, 4);
   }
 }
 
@@ -669,11 +827,15 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       result->blocks[{o.rid, o.cid}] = dense_block(o.m, o.n, s, false);
     }
   } else {
+    // chain outputs (run_sparse_chains) get their arrays once their format is known: a dense window only if they end dense
+    auto chain_out = [&](const OutPlan& o) { return !o.spsp.empty() && o.m > 0 && o.n > 0; };
     size_t total = 0;
-    for (auto& o : plans) total += align_up(static_cast<size_t>(o.m) * o.n * sizeof(double));
+    for (auto& o : plans)
+      if (!chain_out(o)) total += align_up(static_cast<size_t>(o.m) * o.n * sizeof(double));
     Slab slab(ctx, total);
     for (size_t i = 0; i < plans.size(); ++i) {
       auto& o = plans[i];
+      if (chain_out(o)) continue;  // cptr[i] stays null
       Span s = slab.take(static_cast<size_t>(o.m) * o.n * sizeof(double));
       cptr[i] = s.ptr<double>();
       result->blocks[{o.rid, o.cid}] = dense_block(o.m, o.n, s, false);  // product is never transposed (MLMatrix.scala:101)
@@ -1107,7 +1269,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     }
     ctx->stats.gemm_launches += 1;
   }
-  run_sparse_chains(ctx, plans, chains, cptr, planner, result);
+  run_sparse_chains(ctx, plans, chains, cptr, result);
 }
 
 
@@ -1254,6 +1416,8 @@ mr_status mr_matrix_multiply(mr_matrix* left, int64_t leftRowNum, int64_t leftCo
     mr_context* ctx = left->ctx;
     DeviceScope dev(ctx);
     std::lock_guard<std::mutex> lock(ctx->mu);
+    ctx->stats.spgemm_pairs = 0;
+    ctx->stats.spgemm_products = 0;
     if (left->host || right->host)  // C tile by C tile through the device, into a host-resident result (abi_stream.cpp)
       *out = multiply_streamed(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
     else

@@ -320,6 +320,71 @@ struct DenseScatterDesc {
 };
 cudaError_t launch_dense_scatter(const DenseScatterDesc* d_descs, int ndescs, int max_lines, cudaStream_t stream);
 
+// ---- sparse x sparse block products and their partial sums (spgemm.cu) ---------------------------------------------------------
+// A chain: one output block whose partials are all low-density sparse x sparse, computed in a CSC frame (the CSR arrays of a block
+// are the CSC arrays of its transpose, so an all-CSR chain runs as C^T = B^T A^T).  Level l: P_l = L_l * R_l (L: m x kdim,
+// R: kdim x n, both CSC), S <- S + P_l.  Products and sums rounded one by one, zeros dropped after each (see DESIGN section 4.5.1).
+struct SpgemmPair {
+  const int32_t* lp;      // L column pointers (kdim + 1), row indices, values
+  const int32_t* li;
+  const double* lv;
+  const int32_t* rp;      // R column pointers (n + 1), row indices, values
+  const int32_t* ri;
+  const double* rv;
+};
+struct SpgemmChain {
+  int32_t m, n;           // frame dims of the output
+  int32_t pair_begin, levels;
+  int32_t count_off;      // counters of level l: counts[count_off + l] = nnz(P_l), counts[count_off + levels + l] = nnz(S_l) - nnz(S_l-1)
+  int32_t pad;
+  int32_t* colcnt;        // count pass: [n] entries of each column of the final S
+  const int32_t* optr;    // fill pass, sparse output: column pointers [n + 1] ...
+  int32_t* oidx;          // ... row indices (nullptr: dense output) ...
+  double* oval;           // ... values
+  double* dense;          // fill pass, dense output: frame element (r, c) at dense[r * drs + c * dcs], every element written
+  int64_t drs, dcs;
+};
+struct SpgemmItem {       // one CTA's work: columns col0 .. col0 + spgemm_columns_per_item() - 1 of a chain
+  int32_t chain, col0;
+};
+struct SpgemmLaunchShape {
+  int smem_counters;      // per-level counters in shared memory (levels <= this), else global atomics
+  bool acc_in_smem;       // per-warp column accumulators in shared memory, else in the caller's scratch (scratch_bytes)
+  int max_ctas;           // persistent grid
+  size_t scratch_bytes;
+};
+constexpr int kSpgemmMaxSmem = 200 * 1024;
+int spgemm_columns_per_item();
+SpgemmLaunchShape spgemm_shape(int max_m, int max_levels);
+// fill = false: the count pass (colcnt, counts, *d_products += scalar products; counts and products pre-zeroed);
+// fill = true: writes the entries.  Every chain's m <= max_m.
+cudaError_t launch_spgemm(bool fill, const SpgemmItem* d_items, int nitems, const SpgemmChain* d_chains, const SpgemmPair* d_pairs,
+                          int* d_counts, unsigned long long* d_products, void* d_scratch, int max_m, const SpgemmLaunchShape& s,
+                          cudaStream_t stream);
+// out[0] = 0, out[t + 1] = in[0] + ... + in[t], t < n; one CTA per descriptor
+struct ScanDesc {
+  const int32_t* in;
+  int32_t* out;
+  int32_t n;
+  int32_t pad;
+};
+cudaError_t launch_exclusive_scan(const ScanDesc* d_descs, int ndescs, cudaStream_t stream);
+// Stable CSR <-> CSC conversion: the nl input lines (ptr, idx, val; indices < no) become the no lines of the transpose (optr, oidx,
+// oval), indices ascending in every line.  cur: [no] zeroed ints; scans[t] = {cur, optr, no} of descriptor t.
+struct SpTransDesc {
+  const int32_t* ptr;
+  const int32_t* idx;
+  const double* val;
+  int32_t nl, no, nnz;
+  int32_t pad;
+  int32_t* optr;
+  int32_t* oidx;
+  double* oval;
+  int32_t* cur;
+};
+cudaError_t launch_sptrans(const SpTransDesc* d_descs, const ScanDesc* d_scans, int ndescs, int max_nnz, int max_nl, int max_no,
+                           cudaStream_t stream);
+
 // java.util.Random-compatible U(0,1) fill: out[i] = i-th nextDouble() of new Random(seed), batched over blocks
 struct RandDesc {
   double* out;

@@ -16,6 +16,7 @@ run memcheck crtedge "irregular_shapes and (563x563x563-blk200-sparse or 356x300
 run memcheck tf32   "tf32x3_multiply and (300 or 512)"
 run memcheck sparse  "sparse_blocks or sparse_op_sparse or aggregates or project"
 run memcheck spsp    "sparse_times_sparse"
+run memcheck spgemm  "format_pairs_bit_exact and 0.02 or absent_and_empty or block_heights and (blk64 or blk8192) and csc_csr" tests/test_gpu_spgemm.py  # smem and global accumulators, CSR<->CSC conversion, dense and sparse fills
 run memcheck spmm2   "spmm2_vs_oracle and (700 or 0.05 or False) or spmm2_accumulates"               # ragged strips, global-entry path, unsorted rows
 run memcheck sprand  "device_sprand and 512"
 run memcheck grid    "grid_multiply_matches_oracle and 1-4-1024 or sharded_put_block"
