@@ -119,8 +119,9 @@ struct OzakiGemmParams {
   int32_t npad;                // row pitch of the residue planes (bytes)
   int8_t* planes;              // [nmod][Mpad][npad]
   size_t plane_stride;
-  int32_t mod_p[16];
-  double mod_inv[16];          // 1 / p_t
+  uint32_t mod_p[16];
+  uint32_t mod_magic[16];      // floor(2^32 / p_t)
+  uint32_t mod_off[16];        // (-2^31) mod p_t
   // job mode (Ozaki-II engine): the tiles of this launch come from a list (any subset of the buffer's tile grid), the residue
   // planes are compact ([modulus][list index][128 x 256] bytes), and the whole launch is skipped when *gate != 0
   const int2* tile_list;       // (tm, tn) per tile, nullptr = the full tiles_m x tiles_n grid
@@ -173,30 +174,68 @@ __device__ __forceinline__ void consume_item(Acc (&acc)[128], unsigned char* sme
   if (lane == 0) release((it - 1) % STAGES);
 }
 
-// Residues of a warpgroup's exact s32 accumulator into the compact plane of its tile ([128 rows][256 columns] bytes).
-// q = rint(c / p) is exact in fp64 (no integer c / p lies within 1/(2p) of a tie except the true ties of the even modulus 256,
-// where either neighbour is a valid representative).  ADD: the residue byte this SAME thread stored for the lower K half joins
-// the sum before the reduction: ((x mod p) + y) mod p = (x + y) mod p; |y| <= K/2 * 2^14 and x < 256 keep the sum inside int32.
+// v mod p in [0, p) for every |v| < 2^31, on the integer pipes only (no int <-> fp64 conversions, which issue at a quarter of the
+// ALU rate).  w = v + 2^31 is exact as a uint32 (v ^ 0x80000000); magic = floor(2^32 / p) undershoots 2^32 / p by less than one,
+// so umulhi(w, magic) is floor(w / p) or one less and w - q p lies in [0, 2p); one conditional subtract (the unsigned minimum with
+// r - p, which wraps when r < p) gives w mod p, and adding off = (-2^31) mod p with one more subtract gives v mod p.
+__device__ __forceinline__ uint32_t mod_s32(int32_t v, uint32_t pm, uint32_t magic, uint32_t off) {
+  const uint32_t w = static_cast<uint32_t>(v) ^ 0x80000000u;
+  uint32_t r = w - __umulhi(w, magic) * pm;
+  r = min(r, r - pm);
+  r += off;
+  return min(r, r - pm);
+}
+
+// (x + y) mod p byte by byte, for four residue bytes x, y in [0, p)
+__device__ __forceinline__ uint32_t add_mod_bytes(uint32_t x, uint32_t y, uint32_t pm) {
+  uint32_t out = 0;
+#pragma unroll
+  for (int b = 0; b < 4; ++b) {
+    const uint32_t s = ((x >> (8 * b)) & 0xffu) + ((y >> (8 * b)) & 0xffu);
+    out |= min(s, s - pm) << (8 * b);
+  }
+  return out;
+}
+
+// Residues of a warpgroup's exact s32 accumulator into the compact plane of its tile ([128 rows][256 columns] bytes), unsigned in
+// [0, p) as the CRT kernel reads them.  The four lanes of a quad hold two adjacent columns each of the same 8-column group: for
+// every four groups a 4 x 4 transpose of 16-bit pairs over three xor shuffles leaves lane q the whole group 4 b + q of both its
+// rows, written as two 8-byte stores.  ADD: the residue bytes this quad stored for the lower K half are read back (same words) and
+// added modulo p: ((x mod p) + y) mod p = (x + y) mod p.
 template <bool ADD>
-__device__ __forceinline__ void store_residues(const int32_t (&acc)[128], int8_t* tile, int row, int lane, int pm, double pinv) {
-  int8_t* dst = tile + static_cast<size_t>(row) * BN + 2 * (lane & 3);
+__device__ __forceinline__ void store_residues(const int32_t (&acc)[128], int8_t* tile, int row, int lane, uint32_t pm, uint32_t magic,
+                                               uint32_t off) {
+  const int q = lane & 3;
+  uint64_t* dst = reinterpret_cast<uint64_t*>(tile + static_cast<size_t>(row) * BN) + q;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
+  for (int b = 0; b < 8; ++b) {
+    uint32_t x[4];  // x[i]: this lane's two columns of group 4 b + i; row `row` in bits [0, 16), row + 8 in bits [16, 32)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint16_t* d2 = reinterpret_cast<uint16_t*>(dst + h * 8 * BN + 8 * j);
-      const uint32_t prev = ADD ? *d2 : 0u;
-      uint32_t wv = 0;
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        int v = acc[4 * j + 2 * h + e];
-        if (ADD) v += static_cast<int>((prev >> (8 * e)) & 0xffu);
-        int res = v - __double2int_rn(static_cast<double>(v) * pinv) * pm;  // [-p/2, p/2]
-        res += (res >> 31) & pm;                                          // [0, p): the CRT kernel reads unsigned bytes
-        wv |= static_cast<uint32_t>(res) << (8 * e);
-      }
-      *d2 = static_cast<uint16_t>(wv);
+    for (int i = 0; i < 4; ++i) {
+      const int j = 4 * (4 * b + i);
+      x[i] = mod_s32(acc[j], pm, magic, off) | (mod_s32(acc[j + 1], pm, magic, off) << 8) | (mod_s32(acc[j + 2], pm, magic, off) << 16) |
+             (mod_s32(acc[j + 3], pm, magic, off) << 24);
     }
+    uint64_t w0 = 0, w1 = 0;  // group 4 b + q of rows row and row + 8
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int s = q ^ r;  // lane s needs our x[s], and sends us its x[q]
+      uint32_t v = (s & 2) ? ((s & 1) ? x[3] : x[2]) : ((s & 1) ? x[1] : x[0]);
+      if (r) v = __shfl_xor_sync(0xffffffffu, v, r);
+      w0 |= static_cast<uint64_t>(v & 0xffffu) << (16 * s);
+      w1 |= static_cast<uint64_t>(v >> 16) << (16 * s);
+    }
+    uint64_t* d0 = dst + 4 * b;
+    uint64_t* d1 = d0 + BN;  // 8 rows of BN bytes further
+    if (ADD) {
+      const uint64_t y0 = *d0, y1 = *d1;
+      w0 = add_mod_bytes(static_cast<uint32_t>(w0), static_cast<uint32_t>(y0), pm) |
+           (static_cast<uint64_t>(add_mod_bytes(static_cast<uint32_t>(w0 >> 32), static_cast<uint32_t>(y0 >> 32), pm)) << 32);
+      w1 = add_mod_bytes(static_cast<uint32_t>(w1), static_cast<uint32_t>(y1), pm) |
+           (static_cast<uint64_t>(add_mod_bytes(static_cast<uint32_t>(w1 >> 32), static_cast<uint32_t>(y1 >> 32), pm)) << 32);
+    }
+    *d0 = w0;
+    *d1 = w1;
   }
 }
 
@@ -276,7 +315,7 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
         if (p.nmod) {
           // compact planes: [modulus][tile of this launch][128 rows][256 columns], always whole tiles (no guards)
           store_residues<false>(acc, p.planes + static_cast<size_t>(mi) * p.plane_stride + static_cast<size_t>(t) * (BM * BN), trow, lane,
-                                p.mod_p[mi], p.mod_inv[mi]);
+                                p.mod_p[mi], p.mod_magic[mi], p.mod_off[mi]);
           continue;
         }
       }
@@ -334,8 +373,12 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank)
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
   return r;
 }
+// Hands a ring stage back to a producer of the pair.  No cluster-scope release: the only accesses to order are the stage's reads
+// by wgmma (async proxy), which are complete once wgmma.wait_group has returned, and the refill is a TMA write (async proxy again)
+// that the producer issues only after it has observed the barrier's phase flip.  A .release.cluster arrive would make ptxas fence
+// every one of these arrivals at GPU scope (MEMBAR.ALL.GPU, which also waits for the epilogue's outstanding global stores).
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 // the box lands at the same shared-memory offset, and completes the barrier at the same offset, in every CTA of the mask
 __device__ __forceinline__ void tma_2d_multicast(uint32_t dst, const void* tmap, int c0, int c1, uint32_t bar, uint16_t cta_mask) {
@@ -463,8 +506,8 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS_P, 1) o
         mbar_arrive_cluster(empty1 + 8u * static_cast<uint32_t>(st));
       });
       int8_t* tile = p.planes + static_cast<size_t>(mi) * p.plane_stride + static_cast<size_t>(t) * (BM * BN);
-      if (KSPLIT && add) store_residues<true>(acc, tile, trow, lane, p.mod_p[mi], p.mod_inv[mi]);
-      else store_residues<false>(acc, tile, trow, lane, p.mod_p[mi], p.mod_inv[mi]);
+      if (KSPLIT && add) store_residues<true>(acc, tile, trow, lane, p.mod_p[mi], p.mod_magic[mi], p.mod_off[mi]);
+      else store_residues<false>(acc, tile, trow, lane, p.mod_p[mi], p.mod_magic[mi], p.mod_off[mi]);
     }
   }
   __syncthreads();
@@ -1544,8 +1587,10 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
   p.plane_stride = e->plane_stride;
   p.gate = e->bad;
   for (int t = 0; t < e->T; ++t) {
-    p.mod_p[t] = kCrtModuli[t];
-    p.mod_inv[t] = 1.0 / kCrtModuli[t];
+    const uint32_t pm = static_cast<uint32_t>(kCrtModuli[t]);
+    p.mod_p[t] = pm;
+    p.mod_magic[t] = static_cast<uint32_t>((uint64_t{1} << 32) / pm);
+    p.mod_off[t] = (pm - (uint32_t{1} << 31) % pm) % pm;
   }
   for (int off = 0; off < ntiles; off += e->max_tiles) {
     const int cnt = std::min(e->max_tiles, ntiles - off);
