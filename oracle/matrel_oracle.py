@@ -339,7 +339,7 @@ def multiplySparseMatDenseVec(spm: SparseMatrix, dv: DenseMatrix) -> DenseMatrix
     require(dv.numCols == 1, f"vector with more than 1 columns, dv.numCols = {dv.numCols}")
     require(spm.numCols == dv.numRows, "Sparse Mat-Vect dimensions do not match, "
             f"Mat.numCols = {spm.numCols}, Vec.numRows = {dv.numRows}")
-    return DenseMatrix(spm.numRows, 1, spm.to_numpy() @ dv.to_numpy()[:, 0])
+    return gemmsdd(spm, dv)   # the stored entries only, duplicates added: B rows that no entry faces are never read
 
 
 def multiplySparseSparse(ma: SparseMatrix, mb: SparseMatrix) -> MLMatrix:

@@ -18,10 +18,13 @@ run memcheck sparse  "sparse_blocks or sparse_op_sparse or aggregates or project
 run memcheck spsp    "sparse_times_sparse"
 run memcheck spgemm  "format_pairs_bit_exact and 0.02 or absent_and_empty or block_heights and (blk64 or blk8192) and csc_csr" tests/test_gpu_spgemm.py  # smem and global accumulators, CSR<->CSC conversion, dense and sparse fills
 run memcheck spmm2   "spmm2_vs_oracle and (700 or 0.05 or False) or spmm2_accumulates"               # ragged strips, global-entry path, unsorted rows
+run memcheck spmmedge "segment_capacity or extreme_values and pipelined or grid_multiply_rows and sparse and 2-2 or multi_block and 700" tests/test_gpu_spmm_edges.py  # E_CAP +- 1, global window, nnz = 0, ragged strips, grid rows
 run memcheck sprand  "device_sprand and 512"
 run memcheck grid    "grid_multiply_matches_oracle and 1-4-1024 or sharded_put_block"
 run memcheck ksplit  "ksplit_matches_oracle and (1-1-gram or 2-1-odd or 2-4-k3 or 8-1-single)" tests/test_gpu_grid_ksplit.py  # world 1 and multi-GPU, 128-bit and scalar reduce paths
 run memcheck stream  "ragged_absent_and_transposed_blocks and 1 or sparse_times_sparse_keeps" tests/test_gpu_streamed.py  # tiled, double-buffered panels, write-back of dense and sparse C blocks
 run synccheck crt    "crt_multiply_vs_oracle and (256-256-256 or 1024)"
 run synccheck spmm2  "spmm2_vs_oracle and 700"
+run synccheck spmmcap "segment_capacity" tests/test_gpu_spmm_edges.py              # shared-memory and global segments in one tile
+run racecheck spmmcap "segment_capacity" tests/test_gpu_spmm_edges.py
 run racecheck crt2sm "crt_multiply_vs_oracle and 1024"
