@@ -402,6 +402,9 @@ typedef struct mr_stats {
   int64_t spgemm_pairs;     /* block pairs of the most recent mr_matrix_multiply computed by the sparse x sparse kernel (output blocks
                                whose partials are all low-density sparse x sparse; summed over the tiles of a streamed multiply) */
   int64_t spgemm_products;  /* scalar products that kernel performed: sum over its pairs and k of nnz(A(:,k)) * nnz(B(k,:)) */
+  int64_t dspmm_pairs;      /* block pairs of the most recent mr_matrix_multiply computed by the dense x low-density sparse kernel
+                               (summed over the tiles of a streamed multiply) */
+  int64_t dspmm_products;   /* sum over those pairs of stored entries of the sparse block x rows of the dense block */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

@@ -77,6 +77,8 @@ class mr_stats(C.Structure):
         ("stream_d2h_bytes", C.c_int64),
         ("spgemm_pairs", C.c_int64),
         ("spgemm_products", C.c_int64),
+        ("dspmm_pairs", C.c_int64),
+        ("dspmm_products", C.c_int64),
     ]
 
 

@@ -23,6 +23,14 @@ struct OutPlan {
   std::vector<GemmSrc> src;                              // the blocks behind each gemm pair (+ its k-block id)
   std::vector<std::pair<const Block*, const Block*>> spmm;  // sparse x dense pairs
   std::vector<std::pair<const Block*, const Block*>> spsp;  // sparse x sparse, both densities <= 0.1 (ascending k)
+  std::vector<std::pair<const Block*, const Block*>> dspmm; // dense x low-density sparse on the stored entries (dspmm_route)
+  struct Cand {
+    const Block* a;
+    const Block* b;
+    int32_t k;
+    size_t pos;  // its place in `gemm` had it been densified
+  };
+  std::vector<Cand> cand;                                // dense x sparse pairs that may take the route (decided by resolve)
 };
 
 // How LocalMatrix.matrixMultiplication computes one partial product a x b (LocalMatrix.scala:889-914)
@@ -35,6 +43,18 @@ int pair_kind(const Block& a, const Block& b) {
   if (s1 > 0.1) return PAIR_GEMM;   // :903-904
   if (s2 > 0.1) return PAIR_SPMM;   // :906-907
   return PAIR_SPSP;                 // :909-911
+}
+
+// Dense x sparse pairs whose right block is at most this dense are computed from its stored entries (run_dense_sparse) instead of
+// its dense image, when their output block has no pair on the dense engines (DESIGN section 4.5.2: where the value comes from).
+constexpr double kDspmmMaxDensity = 0.02;
+
+// Metadata-only part of the rule: the density and the dims the dense x sparse kernel takes.
+bool dspmm_candidate(const Block& a, const Block& b) {
+  if (!a.dense() || b.dense()) return false;
+  if (b.numRows <= 0 || b.numRows > kSpmmMaxDim || b.numCols < 128 || b.numCols > kSpmmMaxDim) return false;
+  if (a.numRows < 16 || a.numRows > kSpmmMaxDim || (a.numRows % 2) != 0) return false;
+  return b.valuesLen * 1.0 / (static_cast<double>(b.numRows) * b.numCols) <= kDspmmMaxDensity;
 }
 
 struct MultiplyPlanner {
@@ -70,7 +90,9 @@ struct MultiplyPlanner {
                  b.numCols);
     }
     const int kind = pair_kind(a, b);
-    if (kind == PAIR_GEMM) {
+    if (kind == PAIR_GEMM && dspmm_candidate(a, b)) {
+      o.cand.push_back(OutPlan::Cand{&a, &b, k, o.gemm.size()});
+    } else if (kind == PAIR_GEMM) {
       push_gemm(o, dense_of(a), dense_of(b), k);
     } else if (kind == PAIR_SPMM) {
       o.spmm.emplace_back(&a, &dense_of(b));  // the n == 1 SpMV case is the same kernel
@@ -79,7 +101,19 @@ struct MultiplyPlanner {
     }
   }
 
-  void push_gemm(OutPlan& o, const Block& a, const Block& b, int32_t k) {
+  // Once every pair of o is known: its route candidates take the route when o has no pair on the dense engines, else they are
+  // densified into their places among the GEMM pairs (the summation order of the product without the route).
+  void resolve(OutPlan& o) {
+    if (o.gemm.empty()) {
+      for (const OutPlan::Cand& c : o.cand) o.dspmm.emplace_back(c.a, c.b);
+    } else {
+      size_t shift = 0;
+      for (const OutPlan::Cand& c : o.cand) push_gemm(o, *c.a, dense_of(*c.b), c.k, c.pos + shift++);
+    }
+    o.cand.clear();
+  }
+
+  void push_gemm(OutPlan& o, const Block& a, const Block& b, int32_t k, size_t pos = SIZE_MAX) {
     GemmPair p{};
     p.A = a.values.ptr<double>();
     p.B = b.values.ptr<double>();
@@ -89,8 +123,9 @@ struct MultiplyPlanner {
     p.ldb = b.isT ? b.numCols : b.numRows;  // BLAS.scala:336
     p.kdim = a.numCols;
     p.tmA = p.tmB = -1;
-    o.gemm.push_back(p);
-    o.src.push_back(GemmSrc{&a, &b, k});
+    pos = std::min(pos, o.gemm.size());
+    o.gemm.insert(o.gemm.begin() + static_cast<std::ptrdiff_t>(pos), p);
+    o.src.insert(o.src.begin() + static_cast<std::ptrdiff_t>(pos), GemmSrc{&a, &b, k});
   }
 };
 
@@ -785,6 +820,253 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Dense x low-density sparse partials (LocalMatrix.scala:892, dm.multiply(sp.toDense)) from the stored entries of S, after every
+// sparse x dense partial of the same blocks: C (+)= A S as C^T = S^T A^T on spmm2_kernel's dense x sparse variant (spmm.cu).
+// S goes in as its CSC arrays (a CSR block through sptrans), A as a column-major image (row-major or unaligned blocks through an
+// EW_COPY into the scratch).  A flag pass over the A images and a fix-up after the partials give the NaN of a non-finite A(i, k)
+// meeting an implicit zero of S, as the dense image does.  No host synchronisation.
+// ------------------------------------------------------------------------------------------------
+void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<double*>& cptr) {
+  std::vector<size_t> routed;
+  for (size_t i = 0; i < plans.size(); ++i)
+    if (!plans[i].dspmm.empty() && plans[i].m > 0 && plans[i].n > 0) routed.push_back(i);
+  if (routed.empty()) return;
+  // ---- scratch: one buffer (CSC copies of CSR blocks, prepared segments, column-major images, non-finite sets), and one small
+  // zero-filled one (sptrans cursors, the per-block "any non-finite" flags)
+  size_t bytes = 0, zbytes = 0;
+  auto take = [](size_t& total, size_t n) {
+    const size_t off = total;
+    total += align_up(std::max<size_t>(n, 1));
+    return off;
+  };
+  struct SInfo {
+    size_t ptr = 0, idx = 0, val = 0, cur = 0;  // CSC copy of a CSR block
+    size_t ent = 0, rp = 0, seg = 0, kref = 0;
+  };
+  struct AInfo {
+    bool copy = false;
+    size_t img = 0, bits = 0, rowflags = 0, any = 0;
+  };
+  std::map<const Block*, SInfo> sinfo;
+  std::map<const Block*, AInfo> ainfo;
+  std::vector<const Block*> sorder, aorder;
+  for (size_t i : routed)
+    for (auto& pr : plans[i].dspmm) {
+      const Block &a = *pr.first, &sb = *pr.second;
+      wait_ready(ctx, a);
+      wait_ready(ctx, sb);
+      if (!sinfo.count(&sb)) {
+        SInfo v;
+        if (sb.isT) {
+          v.ptr = take(bytes, static_cast<size_t>(sb.numCols + 1) * sizeof(int32_t));
+          v.idx = take(bytes, static_cast<size_t>(sb.valuesLen) * sizeof(int32_t));
+          v.val = take(bytes, static_cast<size_t>(sb.valuesLen) * sizeof(double));
+          v.cur = take(zbytes, static_cast<size_t>(sb.numCols) * sizeof(int32_t));
+        }
+        size_t eo, ro, so, ko;
+        const size_t aux = take(bytes, dspmm_aux_bytes(sb.numCols, sb.numRows, sb.valuesLen, &eo, &ro, &so, &ko));
+        v.ent = aux + eo;
+        v.rp = aux + ro;
+        v.seg = aux + so;
+        v.kref = aux + ko;
+        sinfo.emplace(&sb, v);
+        sorder.push_back(&sb);
+      }
+      if (!ainfo.count(&a)) {
+        AInfo v;
+        v.copy = a.isT || (reinterpret_cast<uintptr_t>(a.values.ptr<double>()) & 15) != 0;
+        if (v.copy) v.img = take(bytes, static_cast<size_t>(a.numRows) * a.numCols * sizeof(double));
+        v.bits = take(bytes, static_cast<size_t>(a.numRows) * DS_KW * sizeof(uint32_t));
+        v.rowflags = take(bytes, static_cast<size_t>((a.numRows + 31) / 32) * sizeof(uint32_t));
+        v.any = take(zbytes, sizeof(int32_t));
+        ainfo.emplace(&a, v);
+        aorder.push_back(&a);
+      }
+    }
+  Buf scratch = std::make_shared<DevBuf>(ctx, bytes), zero = std::make_shared<DevBuf>(ctx, zbytes);
+  CUDA_CHECK(cudaMemsetAsync(zero->p, 0, zbytes, ctx->stream));
+  char* const base = static_cast<char*>(scratch->p);
+  char* const zbase = static_cast<char*>(zero->p);
+  auto csc_of = [&](const Block* sb, const int32_t*& ptr, const int32_t*& idx, const double*& val) {
+    if (sb->isT) {
+      const SInfo& v = sinfo.at(sb);
+      ptr = reinterpret_cast<const int32_t*>(base + v.ptr);
+      idx = reinterpret_cast<const int32_t*>(base + v.idx);
+      val = reinterpret_cast<const double*>(base + v.val);
+    } else {
+      ptr = sb->colPtrs.ptr<int32_t>();
+      idx = sb->rowIndices.ptr<int32_t>();
+      val = sb->values.ptr<double>();
+    }
+  };
+  auto image_of = [&](const Block* a) {
+    const AInfo& v = ainfo.at(a);
+    return v.copy ? reinterpret_cast<const double*>(base + v.img) : a->values.ptr<double>();
+  };
+  // ---- CSR right blocks -> CSC (indices ascending; a repeated coordinate's entries end up next to each other, last stored first)
+  {
+    std::vector<SpTransDesc> td;
+    std::vector<ScanDesc> sd;
+    int max_nnz = 0, max_nl = 0, max_no = 0;
+    for (const Block* sb : sorder) {
+      if (!sb->isT) continue;
+      const SInfo& v = sinfo.at(sb);
+      SpTransDesc d{};
+      d.ptr = sb->colPtrs.ptr<int32_t>();
+      d.idx = sb->rowIndices.ptr<int32_t>();
+      d.val = sb->values.ptr<double>();
+      d.nl = sb->numRows;
+      d.no = sb->numCols;
+      d.nnz = static_cast<int32_t>(sb->valuesLen);
+      d.optr = reinterpret_cast<int32_t*>(base + v.ptr);
+      d.oidx = reinterpret_cast<int32_t*>(base + v.idx);
+      d.oval = reinterpret_cast<double*>(base + v.val);
+      d.cur = reinterpret_cast<int32_t*>(zbase + v.cur);
+      td.push_back(d);
+      sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
+      max_nnz = std::max(max_nnz, d.nnz);
+      max_nl = std::max(max_nl, d.nl);
+      max_no = std::max(max_no, d.no);
+    }
+    if (!td.empty()) {
+      Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
+      CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
+                                max_nnz, max_nl, max_no, ctx->stream));
+      note_launch(ctx, 4);
+    }
+  }
+  // ---- segments of S^T (one prepared copy per right block)
+  {
+    std::vector<DspmmPrep> preps;
+    int max_n = 0, max_k = 0;
+    for (const Block* sb : sorder) {
+      const SInfo& v = sinfo.at(sb);
+      DspmmPrep pp{};
+      const double* val;
+      csc_of(sb, pp.ptrs, pp.idx, val);
+      pp.vals = val;
+      pp.m = sb->numCols;
+      pp.kdim = sb->numRows;
+      pp.ent = reinterpret_cast<unsigned char*>(base + v.ent);
+      pp.rp = reinterpret_cast<int32_t*>(base + v.rp);
+      pp.segoff = reinterpret_cast<int32_t*>(base + v.seg);
+      pp.kref = reinterpret_cast<uint8_t*>(base + v.kref);
+      pp.repeats_reversed = sb->isT ? 1 : 0;  // sptrans_fill_kernel places a row's entries of one column counting down
+      preps.push_back(pp);
+      max_n = std::max(max_n, pp.m);
+      max_k = std::max(max_k, pp.kdim);
+    }
+    Buf d_preps = upload(ctx, preps);
+    CUDA_CHECK(launch_dspmm_prep(static_cast<const DspmmPrep*>(d_preps->p), static_cast<int>(preps.size()), max_n, max_k, ctx->stream));
+    note_launch(ctx);
+  }
+  // ---- column-major images of row-major or unaligned left blocks, and their non-finite sets
+  {
+    std::vector<EwDesc> copies;
+    std::vector<DsFlagDesc> flags;
+    int max_r = 0, max_c = 0, max_m = 0;
+    bool any_t = false;
+    for (const Block* a : aorder) {
+      const AInfo& v = ainfo.at(a);
+      if (v.copy) {
+        EwDesc d{};
+        d.A = a->values.ptr<double>();
+        d.C = reinterpret_cast<double*>(base + v.img);
+        d.rows = a->numRows;
+        d.cols = a->numCols;
+        d.aT = a->isT ? 1 : 0;
+        any_t = any_t || a->isT;
+        max_r = std::max(max_r, d.rows);
+        max_c = std::max(max_c, d.cols);
+        copies.push_back(d);
+      }
+      flags.push_back(DsFlagDesc{image_of(a), a->numRows, a->numCols, reinterpret_cast<uint32_t*>(base + v.bits),
+                                 reinterpret_cast<uint32_t*>(base + v.rowflags), reinterpret_cast<int32_t*>(zbase + v.any)});
+      max_m = std::max(max_m, a->numRows);
+    }
+    if (!copies.empty()) {
+      Buf d_cp = upload(ctx, copies);
+      CUDA_CHECK(launch_ew_batched(EW_COPY, static_cast<const EwDesc*>(d_cp->p), static_cast<int>(copies.size()), max_r, max_c, any_t,
+                                   ctx->stream));
+      note_launch(ctx);
+    }
+    Buf d_fl = upload(ctx, flags);
+    CUDA_CHECK(launch_ds_flags(static_cast<const DsFlagDesc*>(d_fl->p), static_cast<int>(flags.size()), max_m, ctx->stream));
+    note_launch(ctx);
+  }
+  // ---- the partials: one CTA per (256 columns, 64 rows) of an output block, over all of its routed pairs; then the fix-up
+  std::vector<Spmm2Out> outs;
+  std::vector<DspmmPair> pairs;
+  std::vector<DsFixPair> fixes;
+  struct Keyed {
+    int32_t rid, ctile, cid, strip;
+    Spmm2Item it;
+  };
+  std::vector<Keyed> items;
+  for (size_t i : routed) {
+    const OutPlan& o = plans[i];
+    Spmm2Out fo{};
+    fo.C = cptr[i];
+    fo.m = o.n;
+    fo.n = o.m;
+    fo.pair_begin = static_cast<int32_t>(pairs.size());
+    fo.pair_count = static_cast<int32_t>(o.dspmm.size());
+    fo.accumulate = o.spmm.empty() ? 0 : 1;  // the block's sparse x dense partials ran before
+    for (auto& pr : o.dspmm) {
+      const Block &a = *pr.first, &sb = *pr.second;
+      const SInfo& v = sinfo.at(&sb);
+      const AInfo& av = ainfo.at(&a);
+      DspmmPair dp{};
+      dp.ent = reinterpret_cast<const unsigned char*>(base + v.ent);
+      dp.rp = reinterpret_cast<const int32_t*>(base + v.rp);
+      dp.segoff = reinterpret_cast<const int32_t*>(base + v.seg);
+      dp.kref = reinterpret_cast<const uint8_t*>(base + v.kref);
+      dp.A = image_of(&a);
+      dp.kdim = sb.numRows;
+      dp.lda = a.numRows;
+      pairs.push_back(dp);
+      DsFixPair fx{};
+      const double* val;
+      csc_of(&sb, fx.ptr, fx.idx, val);
+      fx.bits = reinterpret_cast<const uint32_t*>(base + av.bits);
+      fx.rowflags = reinterpret_cast<const uint32_t*>(base + av.rowflags);
+      fx.any = reinterpret_cast<const int32_t*>(zbase + av.any);
+      fx.C = cptr[i];
+      fx.m = o.m;
+      fx.n = o.n;
+      fixes.push_back(fx);
+      ctx->stats.dspmm_pairs += 1;
+      ctx->stats.dspmm_products += sb.valuesLen * a.numRows;
+    }
+    const int32_t oi = static_cast<int32_t>(outs.size());
+    outs.push_back(fo);
+    for (int st = 0; st * kSpmm2StripRows < o.n; ++st)
+      for (int ct = 0; ct * kSpmm2TileCols < o.m; ++ct) items.push_back(Keyed{o.rid, ct, o.cid, st, Spmm2Item{oi, st, ct, 0}});
+  }
+  // CTAs resident together read the same 64-row panel of a block row of A: order by (block row, tile, block column, strip)
+  std::sort(items.begin(), items.end(), [](const Keyed& x, const Keyed& y) {
+    return std::tie(x.rid, x.ctile, x.cid, x.strip) < std::tie(y.rid, y.ctile, y.cid, y.strip);
+  });
+  std::vector<Spmm2Item> sorted(items.size());
+  for (size_t t = 0; t < items.size(); ++t) sorted[t] = items[t].it;
+  Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_items = upload(ctx, sorted), d_fix = upload(ctx, fixes);
+  if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
+  CUDA_CHECK(launch_dspmm(static_cast<const Spmm2Item*>(d_items->p), static_cast<int>(sorted.size()), static_cast<const Spmm2Out*>(d_outs->p),
+                          static_cast<const DspmmPair*>(d_pairs->p), ctx->stream));
+  note_launch(ctx);
+  if (ctx->time_kernels) {
+    CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
+    CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
+    float ms = 0.f;
+    CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+    ctx->stats.last_gemm_ms = ms;
+    ctx->stats.gemm_ms_total += ms;
+  }
+  CUDA_CHECK(launch_ds_fixup(static_cast<const DsFixPair*>(d_fix->p), static_cast<int>(fixes.size()), ctx->stream));
+  note_launch(ctx);
+}
+
 void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner& planner, int32_t blkSize,
                   mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows,
                   const MultiplyDecisions* decisions) {
@@ -796,7 +1078,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
   for (size_t i = 0; i < plans.size(); ++i) {
     OutPlan& o = plans[i];
     if (o.spsp.empty()) continue;
-    if (o.gemm.empty() && o.spmm.empty()) {
+    if (o.gemm.empty() && o.spmm.empty() && o.dspmm.empty()) {
       chains.push_back(i);
     } else {
       for (auto& pr : o.spsp) o.spmm.emplace_back(pr.first, &planner.dense_of(*pr.second));
@@ -1187,7 +1469,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       fused_max_n = std::max(fused_max_n, o.n);
       have = true;
     }
-    if (!have) CUDA_CHECK(cudaMemsetAsync(cptr[i], 0, static_cast<size_t>(o.m) * o.n * sizeof(double), ctx->stream));
+    if (!have && o.dspmm.empty()) CUDA_CHECK(cudaMemsetAsync(cptr[i], 0, static_cast<size_t>(o.m) * o.n * sizeof(double), ctx->stream));
   }
   if (!fouts.empty()) {
     Buf d_fo = upload(ctx, fouts), d_fp = upload(ctx, fpairs);
@@ -1269,6 +1551,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     }
     ctx->stats.gemm_launches += 1;
   }
+  run_dense_sparse(ctx, plans, cptr);
   run_sparse_chains(ctx, plans, chains, cptr, result);
 }
 
@@ -1332,6 +1615,7 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
       }
     }
   }
+  for (OutPlan& o : plans) planner.resolve(o);
   std::unique_ptr<mr_matrix> result(out_layout ? new_sharded(ctx, *out_layout, false, false) : new_matrix(ctx));
   if (out_layout) result->blocks.clear();  // only the blocks the product has are present (join semantics); absent ones stay absent
   run_multiply(ctx, plans, planner, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, leftColBlkNum == 1 && rightRowBlkNum == 1,
@@ -1343,16 +1627,21 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
 // ascending k, or the outer-product path with the last duplicate winning), but from metadata: no block is touched.
 MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, const mr_matrix* right, int64_t leftColNum,
                                      int64_t rightRowNum, int32_t blkSize) {
+  using Id = std::pair<int32_t, int32_t>;
   struct Out {
     int32_t m = 0, n = 0;
     bool gemm = false, other = false;
-    int64_t flops = 0;
+    int64_t flops = 0, cand_flops = 0;
+    std::vector<std::pair<Id, Id>> cand;  // dense x sparse pairs that may take the route (MultiplyPlanner::resolve)
   };
-  std::map<std::pair<int32_t, int32_t>, Out> outs;
-  auto pair_into = [](Out& o, const Block& a, const Block& b) {
+  std::map<Id, Out> outs;
+  auto pair_into = [](Out& o, const Id& ia, const Block& a, const Id& ib, const Block& b) {
     o.m = a.numRows;
     o.n = b.numCols;
-    if (pair_kind(a, b) == PAIR_GEMM) {
+    if (pair_kind(a, b) == PAIR_GEMM && dspmm_candidate(a, b)) {
+      o.cand.emplace_back(ia, ib);
+      o.cand_flops += 2ll * a.numRows * b.numCols * a.numCols;
+    } else if (pair_kind(a, b) == PAIR_GEMM) {
       o.gemm = true;
       o.flops += 2ll * a.numRows * b.numCols * a.numCols;
     } else {
@@ -1363,7 +1652,7 @@ MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* lef
     for (auto& l : left->blocks)
       for (auto& r : right->blocks) {
         Out o;
-        pair_into(o, l.second, r.second);
+        pair_into(o, l.first, l.second, r.first, r.second);
         outs[{l.first.first, r.first.second}] = o;
       }
   } else {
@@ -1372,22 +1661,49 @@ MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* lef
     for (auto& l : left->blocks) {
       auto rit = rights.find(l.first.second);
       if (rit == rights.end()) continue;
-      for (auto& jb : rit->second) pair_into(outs[{l.first.first, jb.first}], l.second, *jb.second);
+      for (auto& jb : rit->second) pair_into(outs[{l.first.first, jb.first}], l.first, l.second, {l.first.second, jb.first}, *jb.second);
     }
   }
+  MultiplyDecisions d;
   int64_t flops = 0, tiles128 = 0;
   bool mixed = false;
   for (auto& kv : outs) {
-    const Out& o = kv.second;
+    Out& o = kv.second;
+    if (!o.cand.empty()) {
+      if (o.gemm) {  // densified next to the block's other GEMM pairs
+        o.flops += o.cand_flops;
+        for (auto& c : o.cand) d.ds_dense_right.insert(c.second);
+      } else {
+        o.other = true;
+        for (auto& c : o.cand) {
+          d.ds_left.insert(c.first);
+          d.ds_right.insert(c.second);
+        }
+      }
+    }
     if (!o.gemm || o.m == 0 || o.n == 0) continue;
     flops += o.flops;
     tiles128 += static_cast<int64_t>((o.m + 127) / 128) * ((o.n + 127) / 128);
     mixed = mixed || o.other;  // a block with sparse partials next to dense ones keeps the whole product off the Ozaki-II engine
   }
-  MultiplyDecisions d;
   d.variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
   d.oz2 = !mixed && (ctx->gemm_algo == 4 || (ctx->gemm_algo == 0 && flops >= (1ll << 33)));
   return d;
+}
+
+// Upper bounds of run_dense_sparse's scratch per left block (column-major copy, non-finite sets) and right block (CSC copy of a
+// CSR block, prepared segments).
+size_t dspmm_left_scratch(const Block& a) {
+  return align_up(static_cast<size_t>(a.numRows) * a.numCols * sizeof(double)) +
+         align_up(static_cast<size_t>(a.numRows) * DS_KW * sizeof(uint32_t)) +
+         align_up(static_cast<size_t>((a.numRows + 31) / 32) * sizeof(uint32_t)) + align_up(sizeof(int32_t));
+}
+size_t dspmm_right_scratch(const Block& b) {
+  size_t eo, ro, so, ko, n = align_up(dspmm_aux_bytes(b.numCols, b.numRows, b.valuesLen, &eo, &ro, &so, &ko));
+  if (b.isT)
+    n += align_up(static_cast<size_t>(b.numCols + 1) * sizeof(int32_t)) + align_up(static_cast<size_t>(b.valuesLen) * sizeof(int32_t)) +
+         align_up(static_cast<size_t>(b.valuesLen) * sizeof(double)) + align_up(static_cast<size_t>(b.numCols) * sizeof(int32_t));
+  return n;
 }
 
 size_t oz2_scratch_for(const mr_context* ctx, int32_t blk, int64_t K, int nr, int nc) {
@@ -1418,6 +1734,8 @@ mr_status mr_matrix_multiply(mr_matrix* left, int64_t leftRowNum, int64_t leftCo
     std::lock_guard<std::mutex> lock(ctx->mu);
     ctx->stats.spgemm_pairs = 0;
     ctx->stats.spgemm_products = 0;
+    ctx->stats.dspmm_pairs = 0;
+    ctx->stats.dspmm_products = 0;
     if (left->host || right->host)  // C tile by C tile through the device, into a host-resident result (abi_stream.cpp)
       *out = multiply_streamed(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
     else

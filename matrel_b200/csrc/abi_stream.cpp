@@ -150,11 +150,27 @@ mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNu
     b_col = std::max(b_col, col_dev[kv.first]);
     b_col_dense = std::max(b_col_dense, col_dense[kv.first]);
   }
+  // per block row of A / column of B, what the dense x sparse route allocates for its blocks (b_col_ds: the B blocks' dense images
+  // where they are densified, as before)
+  std::map<int32_t, size_t> a_ds, b_col_ds;
+  for (auto& kv : left->blocks)
+    if (dec.ds_left.count(kv.first)) a_ds[kv.first.first] += dspmm_left_scratch(kv.second);
+  for (auto& kv : right->blocks) {
+    const bool routed = dec.ds_right.count(kv.first) != 0;
+    size_t& n = b_col_ds[kv.first.second];
+    if (!routed || dec.ds_dense_right.count(kv.first)) n += dense_bytes(kv.second);
+    if (routed) n += dspmm_right_scratch(kv.second);
+  }
+  size_t a_ds_max = 0, b_col_ds_max = 0;
+  for (auto& kv : a_ds) a_ds_max = std::max(a_ds_max, kv.second);
+  for (auto& kv : b_col_ds) b_col_ds_max = std::max(b_col_ds_max, kv.second);
   // per block row of A / column of B, the sparse paths of a tile call allocate at most: dense images of sparse A blocks (pairs the
   // reference multiplies densely) and the re-packed CSR segments (bounded by the stored row); dense images of sparse B blocks, and
   // row-major copies of the column-major dense B blocks a sparse x dense kernel reads
-  const size_t a_scratch = a_sparse ? a_row_dense + a_row_fp : 0;
-  const size_t b_scratch = ((b_sparse ? 1 : 0) + (a_sparse ? 1 : 0)) * b_col_dense;
+  // Right blocks of dense x sparse pairs that take the stored-entry route get no dense image: their prepared segments (and CSC
+  // copy) instead, and their left blocks a column-major copy and non-finite sets (DESIGN section 4.5.2).
+  const size_t a_scratch = (a_sparse ? a_row_dense + a_row_fp : 0) + a_ds_max;
+  const size_t b_scratch = (a_sparse ? 1 : 0) * b_col_dense + (b_sparse ? b_col_ds_max : 0);
   // ---- device budget and the tile
   const size_t budget = stream_budget(ctx);
   const size_t c_block = align_up(static_cast<size_t>(max_m) * max_n * sizeof(double));

@@ -14,6 +14,7 @@
 #include <deque>
 #include <functional>
 #include <map>
+#include <set>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -272,6 +273,9 @@ using OutWindowFn = std::function<Span(int32_t rid, int32_t cid)>;
 struct MultiplyDecisions {
   bool oz2 = false;
   int variant = 0;
+  // dense x sparse pairs (ids of their blocks): left and right blocks of the pairs that take the stored-entry route, and right
+  // blocks of the pairs densified next to GEMM pairs (the streamed multiply's scratch bound)
+  std::set<std::pair<int32_t, int32_t>> ds_left, ds_right, ds_dense_right;
 };
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
                          int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr,
@@ -279,6 +283,9 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
 // The decisions multiply_impl would take for left x right, from block metadata only (the blocks may be host-resident).
 MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, const mr_matrix* right, int64_t leftColNum,
                                      int64_t rightRowNum, int32_t blkSize);
+// Scratch the dense x low-density sparse route allocates for one left / right block of its pairs (upper bounds).
+size_t dspmm_left_scratch(const Block& a);
+size_t dspmm_right_scratch(const Block& b);
 // Bytes of Ozaki-II residue scratch multiply_impl allocates for an nr x nc grid of output blocks (the ozaki_scratch_mb rule).
 size_t oz2_scratch_for(const mr_context* ctx, int32_t blk, int64_t K, int nr, int nc);
 // The streamed multiply (abi_stream.cpp): at least one operand is host-resident; the result is host-resident.

@@ -243,6 +243,52 @@ struct SprandDesc {
 int sprand_draws(int64_t nnz);
 cudaError_t launch_sprand(const SprandDesc* d_descs, int nblocks, int max_cols, cudaStream_t stream);
 size_t spmm2_aux_bytes(int m, int kdim, int64_t nnz, size_t* ent_off, size_t* rp_off, size_t* seg_off);
+// ---- dense x low-density sparse partials C (+)= A S on the same kernels, as C^T = S^T A^T (spmm.cu, DESIGN section 4.5.2).  The
+// prepared block is S^T: its CSC arrays (ptrs = column pointers, n + 1; idx = row indices), m = n columns of S, kdim = rows of S.
+struct DspmmPrep {        // Spmm2Prep's fields, then:
+  const int32_t* ptrs;
+  const int32_t* idx;
+  const double* vals;
+  int32_t m, kdim;
+  unsigned char* ent;
+  int32_t* rp;
+  int32_t* segoff;
+  uint8_t* kref;          // out: [strips * chunks][KC] the distinct indices of each segment, by slot (unused slots zero)
+  int32_t repeats_reversed;  // repeated indices of a row are in reverse storage order (a CSR block after launch_sptrans), so the
+                             // first of them is the stored one that counts
+  int32_t pad;
+};
+struct DspmmPair {        // A(i,k) (column-major, lda even, 16-byte aligned) x S(k,j) (prepared)
+  const unsigned char* ent;
+  const int32_t* rp;      // rp[segment][TM + 1]: distinct indices of the segment
+  const int32_t* segoff;
+  const uint8_t* kref;
+  const double* A;
+  int32_t kdim, lda;      // lda = rows of A = Spmm2Out::n
+};
+size_t dspmm_aux_bytes(int n, int kdim, int64_t nnz, size_t* ent_off, size_t* rp_off, size_t* seg_off, size_t* kref_off);
+cudaError_t launch_dspmm_prep(const DspmmPrep* d_preps, int nblocks, int max_n, int max_kdim, cudaStream_t stream);
+// Spmm2Out of an output block C (m x n, column-major): {C, n, m, ...}; items: (out, strip of 256 columns of C, tile of 64 rows)
+cudaError_t launch_dspmm(const Spmm2Item* d_items, int nitems, const Spmm2Out* d_outs, const DspmmPair* d_pairs, cudaStream_t stream);
+constexpr int DS_KW = kSpmmMaxDim / 32;  // words of a row's non-finite set / a column's stored set
+struct DsFlagDesc {       // one left block (column-major image, lda = m)
+  const double* A;
+  int32_t m, kdim;
+  uint32_t* bits;         // out: [m][DS_KW]
+  uint32_t* rowflags;     // out: [(m + 31) / 32]
+  int32_t* any;           // out: 1 when a bit is set (pre-zeroed)
+};
+struct DsFixPair {        // one routed pair, after every partial of its output block
+  const uint32_t* bits;
+  const uint32_t* rowflags;
+  const int32_t* any;
+  const int32_t* ptr;     // CSC of S
+  const int32_t* idx;
+  double* C;              // m x n, column-major
+  int32_t m, n;
+};
+cudaError_t launch_ds_flags(const DsFlagDesc* d_descs, int ndescs, int max_m, cudaStream_t stream);
+cudaError_t launch_ds_fixup(const DsFixPair* d_pairs, int npairs, cudaStream_t stream);
 bool spmm2_encode_b_tmap(void* out128, const double* base, int64_t kdim, int64_t n, int64_t ld);
 cudaError_t launch_spmm2_prep(const Spmm2Prep* d_preps, int nblocks, int max_m, int max_kdim, cudaStream_t stream);
 cudaError_t launch_spmm2(const Spmm2Item* d_items, int nitems, const Spmm2Out* d_outs, const Spmm2Pair* d_pairs, const void* d_tmaps,

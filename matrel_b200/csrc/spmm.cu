@@ -19,10 +19,19 @@
 //   * producer warp + 16 consumer warps, 3-stage full/empty mbarrier ring (a fast warp runs up to two stages ahead of a slow
 //     one); the 256 x 64 result tile is transposed through the (by then idle) stage buffers so that C is written as coalesced
 //     column runs.
+//
+// The same two kernels, instantiated with kDs = true, compute dense x low-density sparse partials C = A S as C^T = S^T A^T:
+// the CSC arrays of S are the CSR arrays of S^T, a column-major A is A^T row-major, and C^T row-major is C column-major.  That
+// variant stages only the columns of A a (strip, chunk) segment references (one 64-row run per distinct k, found by the
+// preparation pass), skips empty segments, keeps only the last of repeated (k, j) entries (SparseMatrix.toArray semantics),
+// and writes C from registers: lane l holds rows 2l, 2l + 1 of one column, so a warp stores a 512-byte run per column.
+// ds_flag_kernel / ds_fixup_kernel give C(i, j) the NaN the densified product gets from a non-finite A(i, k) meeting an
+// implicit zero of column j of S.
 #include <cuda.h>
 
 #include <algorithm>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "kernels.h"
@@ -90,19 +99,62 @@ __device__ __forceinline__ void tma_2d(uint32_t dst, const void* tmap, int c0, i
 // One CTA per sparse block (1024 threads: thread = row, two rows per thread above 1024 are not needed: m <= 1024).
 // Order inside a segment: rows ascending, entries of a row in their CSR storage order (the reference's summation order within
 // the chunk).  segoff[(s * nchunks + q)] = first entry of segment (s, q) in `ent`, segoff[nseg] = nnz.
-__global__ void __launch_bounds__(1024) spmm2_prep_kernel(const Spmm2Prep* __restrict__ preps) {
-  extern __shared__ int32_t cnt[];  // [m_pad][nchunks] counters, then reused as write cursors
+// kDs (dense x sparse): the block is S^T (rows = columns of S); of entries repeating an index in a row only the one toArray keeps
+// counts (kept_entry); every segment's distinct indices get slots in ascending order (kref, count at rp[TM + 1]) and boff
+// addresses the slot.
+constexpr int KW = KC / 32;  // words of a segment's index bitmap
+static_assert(KC / 32 == 4, "kref stores an index inside its chunk as one byte; a producer lane reads its 4 slots as one word");
+template <bool kDs>
+using Spmm2PrepT = typename std::conditional<kDs, DspmmPrep, Spmm2Prep>::type;
+
+template <bool kDs>
+__global__ void __launch_bounds__(1024) spmm2_prep_kernel(const Spmm2PrepT<kDs>* __restrict__ preps) {
+  extern __shared__ int32_t cnt[];  // [m_pad][nchunks] counters, then reused as write cursors (kDs: then [nseg][KW] index bitmaps)
   __shared__ int32_t warp_tot[32];
-  const Spmm2Prep p = preps[blockIdx.x];
+  const Spmm2PrepT<kDs> p = preps[blockIdx.x];
   const int m = p.m, nchunks = (p.kdim + KC - 1) / KC, nstrips = (m + TM - 1) / TM;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int total = nstrips * TM * nchunks;  // counters in (strip, chunk, row-in-strip) order
+  uint32_t* kbits = reinterpret_cast<uint32_t*>(cnt + total);
   for (int i = tid; i < total; i += blockDim.x) cnt[i] = 0;
+  if constexpr (kDs)
+    for (int i = tid; i < nstrips * nchunks * KW; i += blockDim.x) kbits[i] = 0;
   __syncthreads();
   auto slot = [&](int row, int q) { return ((row / TM) * nchunks + q) * TM + (row % TM); };
+  // kDs: is entry e of row [beg, end) the one its index keeps: the last with that index, or the first when p.repeats_reversed
+  // (rows with strictly ascending indices have no repeats)
+  auto kept_entry = [&](int e, int beg, int end, bool ascending) {
+    if constexpr (kDs) {
+      if (ascending) return true;
+      const int c = p.idx[e];
+      for (int f = p.repeats_reversed ? beg : e + 1; f < (p.repeats_reversed ? e : end); ++f)
+        if (p.idx[f] == c) return false;
+    }
+    return true;
+  };
+  auto distinct = [&](int sg) {  // kDs: distinct indices of segment sg
+    int n = 0;
+    for (int w = 0; w < KW; ++w) n += __popc(kbits[sg * KW + w]);
+    return n;
+  };
+  auto ascending_row = [&](int beg, int end) {
+    for (int e = beg + 1; e < end; ++e)
+      if (p.idx[e] <= p.idx[e - 1]) return false;
+    return true;
+  };
   for (int row = tid; row < m; row += blockDim.x) {
     const int beg = p.ptrs[row], end = p.ptrs[row + 1];
-    for (int e = beg; e < end; ++e) atomicAdd(&cnt[slot(row, p.idx[e] / KC)], 1);  // own row only: no contention, plain RMW semantics
+    if constexpr (kDs) {
+      const bool asc = ascending_row(beg, end);
+      for (int e = beg; e < end; ++e) {
+        if (!kept_entry(e, beg, end, asc)) continue;
+        const int col = p.idx[e], q = col / KC, kk = col - q * KC;
+        atomicAdd(&cnt[slot(row, q)], 1);
+        atomicOr(&kbits[((row / TM) * nchunks + q) * KW + (kk >> 5)], 1u << (kk & 31));
+      }
+    } else {
+      for (int e = beg; e < end; ++e) atomicAdd(&cnt[slot(row, p.idx[e] / KC)], 1);  // own row only: no contention, plain RMW semantics
+    }
   }
   __syncthreads();
   // exclusive scan of cnt[0 .. total) (block-wide, chunked by blockDim.x)
@@ -144,20 +196,37 @@ __global__ void __launch_bounds__(1024) spmm2_prep_kernel(const Spmm2Prep* __res
     int v;
     if (r < TM) v = cnt[sg * TM + r] - seg0;
     else v = (sg + 1 < nseg ? cnt[(sg + 1) * TM] : carry) - seg0;  // r == TM (and the padding): segment length
+    if (kDs && r == TM + 1) v = distinct(sg);
     p.rp[i] = v;
   }
+  // kDs: slot -> index inside the chunk
+  auto slot_of = [&](int sg, int kk) {
+    int n = __popc(kbits[sg * KW + (kk >> 5)] & ((1u << (kk & 31)) - 1u));
+    for (int w = 0; w < (kk >> 5); ++w) n += __popc(kbits[sg * KW + w]);
+    return n;
+  };
+  // kDs: the slot table of every segment, all KC bytes written (the producer reads it a word per lane; slots past the segment's
+  // count are zero and never used)
+  if constexpr (kDs)
+    for (int i = tid; i < nseg * KC; i += blockDim.x) {
+      const int sg = i / KC, kk = i % KC;
+      if (kbits[sg * KW + (kk >> 5)] & (1u << (kk & 31))) p.kref[sg * KC + slot_of(sg, kk)] = static_cast<uint8_t>(kk);
+      if (kk >= distinct(sg)) p.kref[sg * KC + kk] = 0;
+    }
   __syncthreads();
   // scatter (cnt becomes the per (row, chunk) write cursor)
   Entry* ent = reinterpret_cast<Entry*>(p.ent);
   for (int row = tid; row < m; row += blockDim.x) {
     const int beg = p.ptrs[row], end = p.ptrs[row + 1];
+    const bool asc = kDs ? ascending_row(beg, end) : true;
     for (int e = beg; e < end; ++e) {
+      if (kDs && !kept_entry(e, beg, end, asc)) continue;
       const int col = p.idx[e];
       const int q = col / KC;
       const int pos = cnt[slot(row, q)]++;
       Entry en;
       en.a = p.vals[e];
-      en.boff = static_cast<uint32_t>(col - q * KC) * (TN * 8);
+      en.boff = static_cast<uint32_t>(kDs ? slot_of((row / TM) * nchunks + q, col - q * KC) : col - q * KC) * (TN * 8);
       en.pad = 0;
       ent[pos] = en;
     }
@@ -183,8 +252,13 @@ __device__ __forceinline__ void lds_f64x2(uint32_t addr, double& x, double& y) {
   asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(x), "=d"(y) : "r"(addr));
 }
 
+template <bool kDs>
+using Spmm2PairT = typename std::conditional<kDs, DspmmPair, Spmm2Pair>::type;
+
+// kDs: out.m / out.n are the dims of C^T (columns of S / rows of A); element C^T(r, c) lives at out.C[r * out.n + c].
+template <bool kDs>
 __global__ void __launch_bounds__(THREADS, 1) spmm2_kernel(const Spmm2Item* __restrict__ items, const Spmm2Out* __restrict__ outs,
-                                                           const Spmm2Pair* __restrict__ pairs, const unsigned char* __restrict__ tmaps) {
+                                                           const Spmm2PairT<kDs>* __restrict__ pairs, const unsigned char* __restrict__ tmaps) {
   extern __shared__ unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((128u - (smem_u32(smem_dyn) & 127u)) & 127u);
   const uint32_t smem_a = smem_u32(smem);
@@ -204,8 +278,50 @@ __global__ void __launch_bounds__(THREADS, 1) spmm2_kernel(const Spmm2Item* __re
   __syncthreads();
 
   if (warp == NCW) {
-    // ===================== producer warp (one elected lane) =====================
-    if (lane == 0) {
+    if constexpr (kDs) {
+      // ===================== producer warp (kDs): one 64-row run of A per distinct k of a non-empty segment, issued by all lanes.
+      // A pair's segment offsets and distinct-index counts are read once (lane q: chunk q), a stage's slot table (4 slots per lane)
+      // before waiting for its buffer, so no dependent global read sits between the wait and the copies.
+      const uint32_t run = static_cast<uint32_t>(min(TN, out.n - col0)) * 8u;  // out.n is even: a multiple of 16 bytes
+      int s = 0;
+      uint32_t ph = 0;
+      for (int p = 0; p < out.pair_count; ++p) {
+        const DspmmPair pr = pairs[out.pair_begin + p];
+        const int nchunks = (pr.kdim + KC - 1) / KC, sg0 = item.strip * nchunks;
+        const int so = lane <= nchunks ? __ldg(pr.segoff + sg0 + lane) : 0;
+        const int nr = lane < nchunks ? __ldg(pr.rp + static_cast<size_t>(sg0 + lane) * RP_PAD + TM + 1) : 0;
+        const int so_next = __shfl_down_sync(0xffffffffu, so, 1);
+        for (uint32_t todo = __ballot_sync(0xffffffffu, lane < nchunks && so_next > so); todo; todo &= todo - 1) {
+          const int q = __ffs(todo) - 1, sg = sg0 + q;
+          const int e0 = __shfl_sync(0xffffffffu, so, q), len = __shfl_sync(0xffffffffu, so_next, q) - e0;
+          const int nref = __shfl_sync(0xffffffffu, nr, q);
+          const uint32_t kw = __ldg(reinterpret_cast<const uint32_t*>(pr.kref + static_cast<size_t>(sg) * KC) + lane);
+          mbar_wait(smem_u32(&bars[NSTAGE + s]), ph ^ 1);
+          const uint32_t st = smem_a + s * STAGE_STRIDE;
+          const uint32_t full = smem_u32(&bars[s]);
+          const uint32_t ent_bytes = len <= E_CAP ? static_cast<uint32_t>(len) * 16u : 0u;
+          if (lane == 0) {
+            mbar_arrive_expect_tx(full, static_cast<uint32_t>(nref) * run + RP_BYTES + ent_bytes);
+            tma_bulk_g2s(st + B_BYTES + ENT_BYTES, pr.rp + static_cast<size_t>(sg) * RP_PAD, RP_BYTES, full);
+            if (ent_bytes) tma_bulk_g2s(st + B_BYTES, pr.ent + static_cast<size_t>(e0) * 16, ent_bytes, full);
+          }
+          __syncwarp();
+#pragma unroll
+          for (int b = 0; b < KC / 32; ++b) {
+            const int t = (KC / 32) * lane + b;
+            if (t < nref) {
+              const int k = q * KC + static_cast<int>((kw >> (8 * b)) & 255u);
+              tma_bulk_g2s(st + t * (TN * 8), pr.A + static_cast<size_t>(k) * pr.lda + col0, run, full);
+            }
+          }
+          if (++s == NSTAGE) {
+            s = 0;
+            ph ^= 1;
+          }
+        }
+      }
+    } else if (lane == 0) {
+      // ===================== producer warp (one elected lane) =====================
       int s = 0;
       uint32_t ph = 0;
       for (int p = 0; p < out.pair_count; ++p) {
@@ -238,9 +354,16 @@ __global__ void __launch_bounds__(THREADS, 1) spmm2_kernel(const Spmm2Item* __re
     int s = 0;
     uint32_t ph = 0;
     for (int p = 0; p < out.pair_count; ++p) {
-      const Spmm2Pair pr = pairs[out.pair_begin + p];
+      const Spmm2PairT<kDs> pr = pairs[out.pair_begin + p];
       const int nchunks = (pr.kdim + KC - 1) / KC;
+      uint32_t nonempty = 0;  // kDs: the chunks the producer stages (lane q reads chunk q's segment offsets)
+      if constexpr (kDs) {
+        const int so = lane <= nchunks ? __ldg(pr.segoff + item.strip * nchunks + lane) : 0;
+        const int so_next = __shfl_down_sync(0xffffffffu, so, 1);
+        nonempty = __ballot_sync(0xffffffffu, lane < nchunks && so_next > so);
+      }
       for (int q = 0; q < nchunks; ++q) {
+        if (kDs && !((nonempty >> q) & 1u)) continue;
         const uint32_t st = smem_a + s * STAGE_STRIDE;
         const uint32_t rp_a = st + B_BYTES + ENT_BYTES;
         const uint32_t bl = st + lane * 16;  // this lane's column pair inside a B row
@@ -301,6 +424,25 @@ __global__ void __launch_bounds__(THREADS, 1) spmm2_kernel(const Spmm2Item* __re
         }
       }
     }
+    if constexpr (kDs) {
+      // ---- epilogue: C^T row r = column row0 + r of C; this lane's two rows of C are adjacent, the warp's 64 a 512-byte run
+      const int rows = min(TM, out.m - row0), c = col0 + 2 * lane;
+#pragma unroll
+      for (int i = 0; i < RPW; ++i) {
+        const int r = warp * RPW + i;
+        if (r < rows && c < out.n) {
+          double2* dst = reinterpret_cast<double2*>(out.C + static_cast<size_t>(out.n) * (row0 + r) + c);
+          double2 v = make_double2(acc[i][0], acc[i][1]);
+          if (out.accumulate) {
+            const double2 o = *dst;
+            v.x = o.x + v.x;
+            v.y = o.y + v.y;
+          }
+          *dst = v;
+        }
+      }
+      return;
+    }
     // ---- epilogue: registers -> shared memory [column][row] -> coalesced column runs of the column-major output block
     asm volatile("bar.sync 1, %0;" ::"r"(NCW * 32) : "memory");  // every consumer has finished reading the stage buffers
     double* Cs = reinterpret_cast<double*>(smem);
@@ -318,6 +460,68 @@ __global__ void __launch_bounds__(THREADS, 1) spmm2_kernel(const Spmm2Item* __re
         double* dst = out.C + static_cast<size_t>(out.m) * (col0 + c) + row0 + r;
         const double v = Cs[c * CS_LD + r];
         *dst = out.accumulate ? *dst + v : v;
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// dense x sparse: the NaN of a non-finite A(i, k) times an implicit zero of column j of S (the densified product's Inf * 0)
+// ------------------------------------------------------------------------------------------------
+// Flag pass: one thread per row of a column-major A (one read of the block).  bits[i * 32 + w] bit b: A(i, 32 w + b) is not
+// finite; rowflags bit i: row i has such an element; *any = 1 when the block has one (pre-zeroed by the caller).
+__device__ __forceinline__ bool nonfinite(double v) { return (__double_as_longlong(v) & 0x7ff0000000000000ll) == 0x7ff0000000000000ll; }
+
+// Grid: x = descriptor (no 65535 limit on the number of blocks), y = 256-row chunk of the block.
+__global__ void __launch_bounds__(256) ds_flag_kernel(const DsFlagDesc* __restrict__ descs) {
+  const DsFlagDesc d = descs[blockIdx.x];
+  const int i = blockIdx.y * 256 + threadIdx.x;
+  if (blockIdx.y * 256 >= d.m) return;
+  bool row_nf = false;
+  if (i < d.m) {
+    for (int w = 0; w < DS_KW; ++w) {
+      uint32_t bits = 0;
+      if (w * 32 < d.kdim) {
+#pragma unroll 8
+        for (int b = 0; b < 32; ++b) {
+          const int k = w * 32 + b;
+          if (k < d.kdim && nonfinite(__ldg(d.A + static_cast<size_t>(k) * d.m + i))) bits |= 1u << b;
+        }
+      }
+      d.bits[static_cast<size_t>(i) * DS_KW + w] = bits;
+      row_nf = row_nf || bits != 0;
+    }
+  }
+  const uint32_t flags = __ballot_sync(0xffffffffu, row_nf);
+  if ((threadIdx.x & 31) == 0 && i < d.m) d.rowflags[i >> 5] = flags;
+  if (row_nf) *d.any = 1;
+}
+
+// Fix-up, after every partial of the blocks: C(i, j) = NaN when some non-finite A(i, k) has no stored (k, j) in S.  Persistent
+// CTAs over the pairs; a pair whose A block is all finite costs one read of its flag.  A warp per column j of S: its stored
+// indices as a 1024-bit set (lane w holds word w), then every flagged row's non-finite set against it.
+static_assert(DS_KW == 32, "lane w holds word w of a 1024-bit set");
+__global__ void __launch_bounds__(256) ds_fixup_kernel(const DsFixPair* __restrict__ pairs, int npairs) {
+  __shared__ uint32_t sb[8][DS_KW];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int p = blockIdx.x; p < npairs; p += gridDim.x) {
+    const DsFixPair f = pairs[p];
+    if (!*f.any) continue;
+    for (int j = warp; j < f.n; j += 8) {
+      sb[warp][lane] = 0;
+      __syncwarp();
+      for (int e = f.ptr[j] + lane; e < f.ptr[j + 1]; e += 32) atomicOr(&sb[warp][f.idx[e] >> 5], 1u << (f.idx[e] & 31));
+      __syncwarp();
+      const uint32_t stored = sb[warp][lane];
+      __syncwarp();
+      for (int i0 = 0; i0 < f.m; i0 += 32) {
+        uint32_t rows = f.rowflags[i0 >> 5];
+        while (rows) {
+          const int i = i0 + __ffs(rows) - 1;
+          rows &= rows - 1;
+          if (__any_sync(0xffffffffu, (f.bits[static_cast<size_t>(i) * DS_KW + lane] & ~stored) != 0) && lane == 0)
+            f.C[static_cast<size_t>(j) * f.m + i] = __longlong_as_double(0x7ff8000000000000ll);
+        }
       }
     }
   }
@@ -508,10 +712,54 @@ cudaError_t launch_spmm2_prep(const Spmm2Prep* d_preps, int nblocks, int max_m, 
   const int nstrips = (max_m + TM - 1) / TM, nchunks = (max_kdim + KC - 1) / KC;
   const size_t smem = static_cast<size_t>(nstrips) * TM * nchunks * sizeof(int32_t);
   static PerDeviceOnce once;
-  cudaError_t e = once.run([&] { return cudaFuncSetAttribute(spmm2_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024); });
+  cudaError_t e = once.run([&] { return cudaFuncSetAttribute(spmm2_prep_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024); });
   if (e != cudaSuccess) return e;
   if (smem > 64 * 1024) return cudaErrorInvalidValue;
-  spmm2_prep_kernel<<<nblocks, 1024, smem, stream>>>(d_preps);
+  spmm2_prep_kernel<false><<<nblocks, 1024, smem, stream>>>(d_preps);
+  return cudaGetLastError();
+}
+
+size_t dspmm_aux_bytes(int n, int kdim, int64_t nnz, size_t* ent_off, size_t* rp_off, size_t* seg_off, size_t* kref_off) {
+  size_t off = spmm2_aux_bytes(n, kdim, nnz, ent_off, rp_off, seg_off);
+  const int nseg = ((n + TM - 1) / TM) * ((kdim + KC - 1) / KC);
+  *kref_off = off;
+  return off + (static_cast<size_t>(nseg) * KC + 255) / 256 * 256;
+}
+
+cudaError_t launch_dspmm_prep(const DspmmPrep* d_preps, int nblocks, int max_n, int max_kdim, cudaStream_t stream) {
+  if (nblocks <= 0) return cudaSuccess;
+  const int nstrips = (max_n + TM - 1) / TM, nchunks = (max_kdim + KC - 1) / KC;
+  const size_t smem = static_cast<size_t>(nstrips) * nchunks * (TM + KW) * sizeof(int32_t);
+  static PerDeviceOnce once;
+  cudaError_t e = once.run([&] { return cudaFuncSetAttribute(spmm2_prep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024); });
+  if (e != cudaSuccess) return e;
+  if (smem > 64 * 1024) return cudaErrorInvalidValue;
+  spmm2_prep_kernel<true><<<nblocks, 1024, smem, stream>>>(d_preps);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_dspmm(const Spmm2Item* d_items, int nitems, const Spmm2Out* d_outs, const DspmmPair* d_pairs, cudaStream_t stream) {
+  if (nitems <= 0) return cudaSuccess;
+  static PerDeviceOnce once;
+  cudaError_t e = once.run([&] { return cudaFuncSetAttribute(spmm2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); });
+  if (e != cudaSuccess) return e;
+  spmm2_kernel<true><<<nitems, THREADS, SMEM_BYTES, stream>>>(d_items, d_outs, d_pairs, nullptr);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ds_flags(const DsFlagDesc* d_descs, int ndescs, int max_m, cudaStream_t stream) {
+  if (ndescs <= 0) return cudaSuccess;
+  ds_flag_kernel<<<dim3(ndescs, (max_m + 255) / 256), 256, 0, stream>>>(d_descs);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ds_fixup(const DsFixPair* d_pairs, int npairs, cudaStream_t stream) {
+  if (npairs <= 0) return cudaSuccess;
+  int dev = 0, sms = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) return e;
+  ds_fixup_kernel<<<std::min(npairs, std::max(sms, 1) * 8), 256, 0, stream>>>(d_pairs, npairs);
   return cudaGetLastError();
 }
 
@@ -538,9 +786,9 @@ cudaError_t launch_spmm2(const Spmm2Item* d_items, int nitems, const Spmm2Out* d
                          cudaStream_t stream) {
   if (nitems <= 0) return cudaSuccess;
   static PerDeviceOnce once;
-  cudaError_t e = once.run([&] { return cudaFuncSetAttribute(spmm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); });
+  cudaError_t e = once.run([&] { return cudaFuncSetAttribute(spmm2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); });
   if (e != cudaSuccess) return e;
-  spmm2_kernel<<<nitems, THREADS, SMEM_BYTES, stream>>>(d_items, d_outs, d_pairs, static_cast<const unsigned char*>(d_tmaps));
+  spmm2_kernel<false><<<nitems, THREADS, SMEM_BYTES, stream>>>(d_items, d_outs, d_pairs, static_cast<const unsigned char*>(d_tmaps));
   return cudaGetLastError();
 }
 

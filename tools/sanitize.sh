@@ -28,3 +28,5 @@ run synccheck spmm2  "spmm2_vs_oracle and 700"
 run synccheck spmmcap "segment_capacity" tests/test_gpu_spmm_edges.py              # shared-memory and global segments in one tile
 run racecheck spmmcap "segment_capacity" tests/test_gpu_spmm_edges.py
 run racecheck crt2sm "crt_multiply_vs_oracle and 1024"
+run memcheck dspmm   "density_around_tau or nonfinite_left or repeated_coordinates or streamed_matches_resident and AB" tests/test_gpu_dspmm.py  # dense x sparse route, flag pass and fix-up
+run racecheck dspmm  "density_around_tau" tests/test_gpu_dspmm.py                 # shared-memory and global segments, empty segments skipped
