@@ -79,6 +79,8 @@ class mr_stats(C.Structure):
         ("spgemm_products", C.c_int64),
         ("dspmm_pairs", C.c_int64),
         ("dspmm_products", C.c_int64),
+        ("ew_sparse_pairs", C.c_int64),
+        ("ew_sparse_entries", C.c_int64),
     ]
 
 

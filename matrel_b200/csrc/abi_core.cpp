@@ -135,81 +135,6 @@ Block densify(mr_context* ctx, const Block& s) {
 const char* type_name(const Block& b) { return b.dense() ? "DenseMatrix" : "SparseMatrix"; }
 
 int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
-// ------------------------------------------------------------------------------------------------
-// dense window -> CSC compaction (DenseMatrix.toSparse, MLMatrix.scala:392-420), batched
-// ------------------------------------------------------------------------------------------------
-// Per-column counts of entries != 0.0 (NaN counts, as in the reference's `arr(i) != 0`): one launch + one sync.
-std::vector<std::vector<int32_t>> column_counts(mr_context* ctx, const std::vector<DenseWin>& wins) {
-  std::vector<std::vector<int32_t>> out(wins.size());
-  if (wins.empty()) return out;
-  size_t ncols_total = 0;
-  int maxc = 0;
-  for (auto& w : wins) {
-    ncols_total += static_cast<size_t>(w.cols);
-    maxc = std::max(maxc, w.cols);
-  }
-  Buf counts = std::make_shared<DevBuf>(ctx, std::max<size_t>(ncols_total * sizeof(int32_t), 16));
-  std::vector<CscDesc> cd(wins.size());
-  size_t off = 0;
-  for (size_t i = 0; i < wins.size(); ++i) {
-    cd[i] = CscDesc{wins[i].p, wins[i].rows, wins[i].cols, static_cast<int32_t*>(counts->p) + off, nullptr, nullptr, nullptr};
-    off += static_cast<size_t>(wins[i].cols);
-  }
-  Buf dcd = upload(ctx, cd);
-  CUDA_CHECK(launch_csc_count(static_cast<const CscDesc*>(dcd->p), static_cast<int>(cd.size()), maxc, ctx->stream));
-  note_launch(ctx);
-  std::vector<int32_t> h(ncols_total);
-  if (ncols_total) {
-    CUDA_CHECK(cudaMemcpyAsync(h.data(), counts->p, ncols_total * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    ctx->stats.d2h_bytes += static_cast<int64_t>(ncols_total * sizeof(int32_t));
-  }
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  off = 0;
-  for (size_t i = 0; i < wins.size(); ++i) {
-    out[i].assign(h.begin() + static_cast<std::ptrdiff_t>(off), h.begin() + static_cast<std::ptrdiff_t>(off + wins[i].cols));
-    off += static_cast<size_t>(wins[i].cols);
-  }
-  return out;
-}
-
-int64_t total_count(const std::vector<int32_t>& counts) {
-  int64_t n = 0;
-  for (int32_t c : counts) n += c;
-  return n;
-}
-
-// CSC blocks (isTransposed = false) of the windows, given their column counts: one launch.
-std::vector<Block> compact_csc(mr_context* ctx, const std::vector<DenseWin>& wins, const std::vector<std::vector<int32_t>>& counts) {
-  std::vector<Block> out;
-  std::vector<CscDesc> fill;
-  int maxc = 0;
-  for (size_t i = 0; i < wins.size(); ++i) {
-    const int rows = wins[i].rows, cols = wins[i].cols;
-    std::vector<int32_t> ptrs(static_cast<size_t>(cols) + 1, 0);
-    for (int c = 0; c < cols; ++c) ptrs[c + 1] = ptrs[c] + counts[i][c];
-    const int64_t nnz = ptrs[cols];
-    Block sb;
-    sb.type = 0;
-    sb.numRows = rows;
-    sb.numCols = cols;
-    sb.isT = false;
-    sb.valuesLen = nnz;
-    sb.colPtrsLen = cols + 1;
-    sb.colPtrs = upload_raw(ctx, ptrs.data(), ptrs.size() * sizeof(int32_t));
-    sb.rowIndices = Span{std::make_shared<DevBuf>(ctx, std::max<size_t>(nnz * sizeof(int32_t), 16)), 0};
-    sb.values = Span{std::make_shared<DevBuf>(ctx, std::max<size_t>(nnz * sizeof(double), 16)), 0};
-    fill.push_back(CscDesc{wins[i].p, rows, cols, nullptr, sb.colPtrs.ptr<int32_t>(), sb.rowIndices.ptr<int32_t>(),
-                           sb.values.ptr<double>()});
-    maxc = std::max(maxc, cols);
-    out.push_back(std::move(sb));
-  }
-  if (!fill.empty()) {
-    Buf dfill = upload(ctx, fill);
-    CUDA_CHECK(launch_csc_fill(static_cast<const CscDesc*>(dfill->p), static_cast<int>(fill.size()), maxc, ctx->stream));
-    note_launch(ctx);
-  }
-  return out;
-}
 mr_matrix* new_matrix(mr_context* ctx) {
   auto* m = new mr_matrix;
   m->ctx = ctx;

@@ -24,13 +24,13 @@ struct EwBatch {
   mr_context* ctx;
   int op;
   std::vector<EwDesc> descs;
-  std::vector<Block> keep;  // densified temporaries
+  std::vector<Block> keep;  // densified temporaries (rank-one update)
   std::vector<std::pair<std::pair<int32_t, int32_t>, std::pair<int32_t, int32_t>>> shapes;  // key -> (rows, cols)
   int max_rows = 0, max_cols = 0;
   bool any_T = false;
   size_t total = 0;
-  std::vector<size_t> sparse_rule;  // indices of results that follow the sparse (op) sparse output-format rule
 
+  // a or b may be null: an absent operand (0.0 everywhere) of EW_ADD / EW_MUL / EW_DIV
   void add(std::pair<int32_t, int32_t> key, const Block* a, const Block* b, const double* y, int rows, int cols) {
     EwDesc d{};
     d.A = a ? a->values.ptr<double>() : nullptr;
@@ -61,30 +61,182 @@ struct EwBatch {
     CUDA_CHECK(launch_ew_batched(op, static_cast<const EwDesc*>(d->p), static_cast<int>(descs.size()), max_rows,
                                  max_cols, any_T, ctx->stream));
     note_launch(ctx);
-    if (!sparse_rule.empty()) apply_sparse_rule(result);
-  }
-
-  // LocalMatrix.addSparseSparse / elementWiseOpSparseSparse output format (LocalMatrix.scala:74-139, 521-602): the
-  // dense result is converted with toSparse (CSC, isTransposed = false) iff rows*cols > 2*nnz + cols + 1, where nnz
-  // counts entries != 0.0 (NaN included).  Both the transposed and the native branch reduce to this rule.
-  void apply_sparse_rule(mr_matrix* result) {
-    std::vector<DenseWin> wins;
-    for (size_t bi : sparse_rule) wins.push_back(DenseWin{descs[bi].C, shapes[bi].second.first, shapes[bi].second.second});
-    const auto counts = column_counts(ctx, wins);
-    std::vector<DenseWin> chosen;
-    std::vector<std::vector<int32_t>> chosen_counts;
-    std::vector<std::pair<int32_t, int32_t>> keys;
-    for (size_t i = 0; i < wins.size(); ++i) {
-      if (static_cast<int64_t>(wins[i].rows) * wins[i].cols > 2 * total_count(counts[i]) + wins[i].cols + 1) {
-        chosen.push_back(wins[i]);
-        chosen_counts.push_back(counts[i]);
-        keys.push_back(shapes[sparse_rule[i]].first);
-      }
-    }
-    std::vector<Block> fresh = compact_csc(ctx, chosen, chosen_counts);
-    for (size_t i = 0; i < fresh.size(); ++i) result->blocks[keys[i]] = std::move(fresh[i]);  // replaces the dense window
   }
 };
+
+// ------------------------------------------------------------------------------------------------
+// sparse (+) sparse on the stored entries (sparse_ew.cu, DESIGN section 4.5.3): a count pass over every pair of the call, one
+// host synchronisation for the per-pair totals, the reference's output rule, exactly sized results from one slab, a fill pass.
+// ------------------------------------------------------------------------------------------------
+struct SparsePair {
+  std::pair<int32_t, int32_t> key;
+  const Block* a;
+  const Block* b;
+};
+
+void sparse_sparse_join(mr_context* ctx, int op, const std::vector<SparsePair>& jobs, mr_matrix* result) {
+  if (jobs.empty()) return;
+  const size_t np = jobs.size();
+  // ---- CSR operands through sptrans, once per block: scratch = cursors (zeroed), then the CSC arrays
+  struct Conv {
+    size_t ptr, idx, val, cur;
+  };
+  std::map<const Block*, Conv> conv;
+  size_t cur_bytes = 0, conv_bytes = 0;
+  for (auto& j : jobs)
+    for (const Block* b : {j.a, j.b})
+      if (b->isT && !conv.count(b)) {
+        Conv v{};
+        v.cur = cur_bytes;
+        cur_bytes += align_up(static_cast<size_t>(b->numCols) * sizeof(int32_t));
+        v.ptr = conv_bytes;
+        conv_bytes += align_up(static_cast<size_t>(b->numCols + 1) * sizeof(int32_t));
+        v.idx = conv_bytes;
+        conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(int32_t));
+        v.val = conv_bytes;
+        conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(double));
+        conv.emplace(b, v);
+      }
+  Buf cbuf;
+  if (!conv.empty()) {
+    cbuf = std::make_shared<DevBuf>(ctx, cur_bytes + conv_bytes);
+    CUDA_CHECK(cudaMemsetAsync(cbuf->p, 0, cur_bytes, ctx->stream));
+    char* base = static_cast<char*>(cbuf->p);
+    std::vector<SpTransDesc> td;
+    std::vector<ScanDesc> sd;
+    int max_nnz = 0, max_nl = 0, max_no = 0;
+    for (auto& kv : conv) {
+      const Block* b = kv.first;
+      const Conv& v = kv.second;
+      SpTransDesc d{};
+      d.ptr = b->colPtrs.ptr<int32_t>();
+      d.idx = b->rowIndices.ptr<int32_t>();
+      d.val = b->values.ptr<double>();
+      d.nl = b->numRows;
+      d.no = b->numCols;
+      d.nnz = static_cast<int32_t>(b->valuesLen);
+      d.optr = reinterpret_cast<int32_t*>(base + cur_bytes + v.ptr);
+      d.oidx = reinterpret_cast<int32_t*>(base + cur_bytes + v.idx);
+      d.oval = reinterpret_cast<double*>(base + cur_bytes + v.val);
+      d.cur = reinterpret_cast<int32_t*>(base + v.cur);
+      td.push_back(d);
+      sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
+      max_nnz = std::max(max_nnz, d.nnz);
+      max_nl = std::max(max_nl, d.nl);
+      max_no = std::max(max_no, d.no);
+    }
+    Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
+    CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
+                              max_nnz, max_nl, max_no, ctx->stream));
+    note_launch(ctx, 4);
+  }
+  // ---- the pairs in the CSC frame
+  size_t col_total = 0;
+  for (auto& j : jobs) col_total += static_cast<size_t>(j.a->numCols);
+  const size_t tot_off = 0, cnt_off = align_up(np * sizeof(unsigned long long));
+  Buf meta = std::make_shared<DevBuf>(ctx, cnt_off + std::max<size_t>(col_total, 1) * sizeof(int32_t));
+  CUDA_CHECK(cudaMemsetAsync(meta->p, 0, cnt_off, ctx->stream));
+  auto* d_total = reinterpret_cast<unsigned long long*>(static_cast<char*>(meta->p) + tot_off);
+  int32_t* d_colcnt = reinterpret_cast<int32_t*>(static_cast<char*>(meta->p) + cnt_off);
+  std::vector<SpEwPair> pairs(np);
+  int max_rows = 0, max_cols = 0;
+  size_t coff = 0;
+  for (size_t i = 0; i < np; ++i) {
+    const Block* a = jobs[i].a;
+    const Block* b = jobs[i].b;
+    const bool native = !a->isT && !b->isT;
+    SpEwPair& q = pairs[i];
+    auto csc_of = [&](const Block* x, const int32_t*& p, const int32_t*& ix, const double*& v, uint8_t& mode) {
+      if (x->isT) {
+        const Conv& cv = conv.at(x);
+        char* base = static_cast<char*>(cbuf->p) + cur_bytes;
+        p = reinterpret_cast<const int32_t*>(base + cv.ptr);
+        ix = reinterpret_cast<const int32_t*>(base + cv.idx);
+        v = reinterpret_cast<const double*>(base + cv.val);
+        mode = SPEW_FIRST;
+      } else {
+        p = x->colPtrs.ptr<int32_t>();
+        ix = x->rowIndices.ptr<int32_t>();
+        v = x->values.ptr<double>();
+        mode = native ? SPEW_SUM : SPEW_LAST;
+      }
+    };
+    csc_of(a, q.ap, q.ai, q.av, q.amode);
+    csc_of(b, q.bp, q.bi, q.bv, q.bmode);
+    q.rows = a->numRows;
+    q.cols = a->numCols;
+    q.native = native ? 1 : 0;
+    q.colcnt = d_colcnt + coff;
+    q.total = d_total + i;
+    coff += static_cast<size_t>(q.cols);
+    max_rows = std::max(max_rows, q.rows);
+    max_cols = std::max(max_cols, q.cols);
+    ctx->stats.ew_sparse_pairs += 1;
+    ctx->stats.ew_sparse_entries += a->valuesLen + b->valuesLen;
+  }
+  // ---- count pass, the per-pair totals
+  const SpEwLaunchShape shape = sparse_ew_shape(max_rows);
+  Buf scratch = shape.scratch_bytes ? std::make_shared<DevBuf>(ctx, shape.scratch_bytes) : nullptr;
+  Buf d_pairs = upload(ctx, pairs);
+  CUDA_CHECK(launch_sparse_ew(op, false, static_cast<const SpEwPair*>(d_pairs->p), static_cast<int>(np), max_rows, max_cols,
+                              scratch ? scratch->p : nullptr, shape, ctx->stream));
+  note_launch(ctx);
+  std::vector<unsigned long long> nnz(np);
+  CUDA_CHECK(cudaMemcpyAsync(nnz.data(), d_total, np * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+  ctx->stats.d2h_bytes += static_cast<int64_t>(np * sizeof(unsigned long long));
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  // ---- the reference's output rule (LocalMatrix.scala:82-88, :131-138): CSC (isTransposed = false) iff rows * cols > 2 nnz + cols + 1
+  std::vector<bool> sparse_out(np);
+  size_t bytes = 0;
+  for (size_t i = 0; i < np; ++i) {
+    const SpEwPair& q = pairs[i];
+    sparse_out[i] = static_cast<int64_t>(q.rows) * q.cols > 2 * static_cast<int64_t>(nnz[i]) + q.cols + 1;
+    if (sparse_out[i])
+      bytes += align_up((static_cast<size_t>(q.cols) + 1) * sizeof(int32_t)) + align_up(nnz[i] * sizeof(int32_t)) +
+               align_up(nnz[i] * sizeof(double));
+    else
+      bytes += align_up(static_cast<size_t>(q.rows) * q.cols * sizeof(double));
+  }
+  Slab slab(ctx, bytes);
+  std::vector<ScanDesc> scans;
+  for (size_t i = 0; i < np; ++i) {
+    SpEwPair& q = pairs[i];
+    Block& out = result->blocks[jobs[i].key];
+    if (!sparse_out[i]) {
+      Span s = slab.take(static_cast<size_t>(q.rows) * q.cols * sizeof(double));
+      q.dense = s.ptr<double>();
+      out = dense_block(q.rows, q.cols, s, false);
+      continue;
+    }
+    Span ptr = slab.take((static_cast<size_t>(q.cols) + 1) * sizeof(int32_t)), idx = slab.take(nnz[i] * sizeof(int32_t)),
+         val = slab.take(nnz[i] * sizeof(double));
+    q.optr = ptr.ptr<int32_t>();
+    q.oidx = idx.ptr<int32_t>();
+    q.oval = val.ptr<double>();
+    scans.push_back(ScanDesc{q.colcnt, ptr.ptr<int32_t>(), q.cols, 0});
+    Block b;
+    b.type = 0;
+    b.numRows = q.rows;
+    b.numCols = q.cols;
+    b.isT = false;
+    b.valuesLen = static_cast<int64_t>(nnz[i]);
+    b.colPtrsLen = q.cols + 1;
+    b.colPtrs = ptr;
+    b.rowIndices = idx;
+    b.values = val;
+    out = std::move(b);
+  }
+  // ---- fill pass
+  if (!scans.empty()) {
+    Buf d_scans = upload(ctx, scans);
+    CUDA_CHECK(launch_exclusive_scan(static_cast<const ScanDesc*>(d_scans->p), static_cast<int>(scans.size()), ctx->stream));
+    note_launch(ctx);
+  }
+  Buf d_pairs2 = upload(ctx, pairs);
+  CUDA_CHECK(launch_sparse_ew(op, true, static_cast<const SpEwPair*>(d_pairs2->p), static_cast<int>(np), max_rows, max_cols,
+                              scratch ? scratch->p : nullptr, shape, ctx->stream));
+  note_launch(ctx);
+}
 
 void check_block_dims_add(const Block& a, const Block& b) {
   // LocalMatrix.add (LocalMatrix.scala:36-41)
@@ -104,13 +256,13 @@ void check_block_dims_ew(const Block& a, const Block& b) {
 
 void elementwise_join(int op, mr_matrix* left, mr_matrix* right, mr_matrix* result) {
   mr_context* ctx = left->ctx;
-  EwBatch batch{ctx, op};
-  batch.keep.reserve(2 * (left->blocks.size() + right->blocks.size()) + 2);
-  auto dense_view = [&](const Block& b) -> const Block* {
-    if (b.dense()) return &b;
-    batch.keep.push_back(densify(ctx, b));
-    return &batch.keep.back();
-  };
+  ctx->stats.ew_sparse_pairs = 0;
+  ctx->stats.ew_sparse_entries = 0;
+  EwBatch batch{ctx, op};           // dense (+) dense, and the unstored positions of dense (+) sparse
+  std::vector<DsEwDesc> scatter;    // dense (+) sparse: the stored positions, after the batch (its index in batch.descs in .C)
+  std::vector<size_t> scatter_at;
+  std::vector<SparsePair> spsp;     // sparse (+) sparse
+  int max_lines = 0;
   for (auto& kv : left->blocks) {
     auto it = right->blocks.find(kv.first);
     if (it == right->blocks.end()) {
@@ -121,18 +273,49 @@ void elementwise_join(int op, mr_matrix* left, mr_matrix* right, mr_matrix* resu
     const Block& b = it->second;
     if (op == EW_ADD) check_block_dims_add(a, b);
     else check_block_dims_ew(a, b);
-    const bool both_sparse = !a.dense() && !b.dense();
-    const Block* x = dense_view(a);
-    const Block* y = dense_view(b);
-    // defect B4 (LocalMatrix.scala:474,487): (Sparse, Dense) swaps the operands; visible for divide only
-    if (op == EW_DIV && !a.dense() && b.dense() && ctx->compat_bugs) std::swap(x, y);
-    batch.add(kv.first, x, y, nullptr, a.numRows, a.numCols);
-    if (both_sparse) batch.sparse_rule.push_back(batch.descs.size() - 1);
+    if (!a.dense() && !b.dense()) {
+      spsp.push_back(SparsePair{kv.first, &a, &b});
+      continue;
+    }
+    if (a.dense() && b.dense()) {
+      batch.add(kv.first, &a, &b, nullptr, a.numRows, a.numCols);
+      continue;
+    }
+    // dense (+) sparse: op(x, y) with the sparse operand absent from the batch; defect B4 (LocalMatrix.scala:474,487): (Sparse,
+    // Dense) swaps the operands, visible for divide only
+    const Block& s = a.dense() ? b : a;
+    const Block& d = a.dense() ? a : b;
+    const bool sparse_left = !a.dense() && !(op == EW_DIV && ctx->compat_bugs);
+    if (sparse_left) batch.add(kv.first, nullptr, &d, nullptr, a.numRows, a.numCols);
+    else batch.add(kv.first, &d, nullptr, nullptr, a.numRows, a.numCols);
+    ctx->stats.ew_sparse_pairs += 1;
+    ctx->stats.ew_sparse_entries += s.valuesLen;
+    if (s.valuesLen == 0) continue;
+    DsEwDesc e{};
+    e.ptr = s.colPtrs.ptr<int32_t>();
+    e.idx = s.rowIndices.ptr<int32_t>();
+    e.val = s.values.ptr<double>();
+    e.D = d.values.ptr<double>();
+    e.rows = a.numRows;
+    e.cols = a.numCols;
+    e.sT = s.isT ? 1 : 0;
+    e.dT = d.isT ? 1 : 0;
+    e.sparse_left = sparse_left ? 1 : 0;
+    scatter.push_back(e);
+    scatter_at.push_back(batch.descs.size() - 1);
+    max_lines = std::max(max_lines, s.isT ? s.numRows : s.numCols);
   }
   if (op == EW_ADD)
     for (auto& kv : right->blocks)
       if (!left->blocks.count(kv.first)) result->blocks[kv.first] = kv.second;
   batch.run(result);
+  if (!scatter.empty()) {
+    for (size_t i = 0; i < scatter.size(); ++i) scatter[i].C = batch.descs[scatter_at[i]].C;
+    Buf d = upload(ctx, scatter);
+    CUDA_CHECK(launch_sparse_ew_scatter(op, static_cast<const DsEwDesc*>(d->p), static_cast<int>(scatter.size()), max_lines, ctx->stream));
+    note_launch(ctx);
+  }
+  sparse_sparse_join(ctx, op, spsp, result);
 }
 
 void map_values(int op, mr_matrix* a, double alpha, mr_matrix* result) {

@@ -36,12 +36,13 @@ __device__ __forceinline__ void st_stream(double2* p, double2 v) {
 constexpr int FLAT_THREADS = 256;
 constexpr int FLAT_UNROLL = 4;
 
-// Both operands share C's layout: pure streaming.
+// Both operands share C's layout: pure streaming.  A null A or B (EW_ADD/MUL/DIV) is an absent operand: 0.0.
 template <int OP>
 __global__ void __launch_bounds__(FLAT_THREADS) ew_flat_kernel(const EwDesc* __restrict__ descs) {
   const EwDesc d = descs[blockIdx.y];
   const int64_t n = static_cast<int64_t>(d.rows) * d.cols;
-  const bool has_b = (OP != EW_COPY);
+  const bool has_a = d.A != nullptr;
+  const bool has_b = (OP != EW_COPY) && d.B != nullptr;
   const bool vec_ok = ((reinterpret_cast<uintptr_t>(d.A) | reinterpret_cast<uintptr_t>(d.C) |
                         (has_b ? reinterpret_cast<uintptr_t>(d.B) : 0)) & 15) == 0;
   const int64_t nvec = vec_ok ? (n >> 1) : 0;
@@ -53,23 +54,20 @@ __global__ void __launch_bounds__(FLAT_THREADS) ew_flat_kernel(const EwDesc* __r
   for (; i + (FLAT_UNROLL - 1) * stride < nvec; i += FLAT_UNROLL * stride) {
     double2 a[FLAT_UNROLL], b[FLAT_UNROLL];
 #pragma unroll
-    for (int u = 0; u < FLAT_UNROLL; ++u) a[u] = ld_stream(A2 + i + u * stride);
-    if (has_b) {
+    for (int u = 0; u < FLAT_UNROLL; ++u) a[u] = has_a ? ld_stream(A2 + i + u * stride) : make_double2(0.0, 0.0);
 #pragma unroll
-      for (int u = 0; u < FLAT_UNROLL; ++u) b[u] = ld_stream(B2 + i + u * stride);
-    }
+    for (int u = 0; u < FLAT_UNROLL; ++u) b[u] = has_b ? ld_stream(B2 + i + u * stride) : make_double2(0.0, 0.0);
 #pragma unroll
     for (int u = 0; u < FLAT_UNROLL; ++u) {
       double2 c;
-      c.x = ew_apply<OP>(a[u].x, has_b ? b[u].x : 0.0);
-      c.y = ew_apply<OP>(a[u].y, has_b ? b[u].y : 0.0);
+      c.x = ew_apply<OP>(a[u].x, b[u].x);
+      c.y = ew_apply<OP>(a[u].y, b[u].y);
       st_stream(C2 + i + u * stride, c);
     }
   }
   for (; i < nvec; i += stride) {
-    const double2 a = ld_stream(A2 + i);
-    double2 b = make_double2(0.0, 0.0);
-    if (has_b) b = ld_stream(B2 + i);
+    const double2 a = has_a ? ld_stream(A2 + i) : make_double2(0.0, 0.0);
+    const double2 b = has_b ? ld_stream(B2 + i) : make_double2(0.0, 0.0);
     double2 c;
     c.x = ew_apply<OP>(a.x, b.x);
     c.y = ew_apply<OP>(a.y, b.y);
@@ -77,7 +75,7 @@ __global__ void __launch_bounds__(FLAT_THREADS) ew_flat_kernel(const EwDesc* __r
   }
   // scalar tail (odd n, or unaligned borrowed pointers)
   for (int64_t j = 2 * nvec + static_cast<int64_t>(blockIdx.x) * FLAT_THREADS + threadIdx.x; j < n; j += stride)
-    d.C[j] = ew_apply<OP>(d.A[j], has_b ? d.B[j] : 0.0);
+    d.C[j] = ew_apply<OP>(has_a ? d.A[j] : 0.0, has_b ? d.B[j] : 0.0);
 }
 
 // Layout-mixing path: 32x32 tile, 32x8 threads; output (r = r0 + tx, c = c0 + ty + 8j).
@@ -138,7 +136,7 @@ __global__ void __launch_bounds__(256) ew_tiled_kernel(const EwDesc* __restrict_
     return;
   }
   if (d.A != nullptr) load_tile(d.A, d.aT != 0, d.rows, d.cols, r0, c0, sm, a);
-  if (OP == EW_ADD || OP == EW_MUL || OP == EW_DIV) load_tile(d.B, d.bT != 0, d.rows, d.cols, r0, c0, sm, b);
+  if ((OP == EW_ADD || OP == EW_MUL || OP == EW_DIV) && d.B != nullptr) load_tile(d.B, d.bT != 0, d.rows, d.cols, r0, c0, sm, b);
   const int r = r0 + tx;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -348,40 +346,6 @@ __global__ void __launch_bounds__(256) java_rand_kernel(const RandDesc* __restri
     s = (s * 0x5DEECE66Dull + 0xBull) & MASK;
     const uint64_t lo = s >> 21;  // next(27)
     d.out[i] = static_cast<double>((hi << 27) + lo) * (1.0 / 9007199254740992.0);
-  }
-}
-
-// one warp per column: count entries with v != 0.0 (NaN != 0.0 is true, like the JVM)
-__global__ void __launch_bounds__(256) csc_count_kernel(const CscDesc* __restrict__ descs) {
-  const CscDesc d = descs[blockIdx.y];
-  const int col = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (col >= d.cols) return;
-  const double* c = d.dense + static_cast<size_t>(d.rows) * col;
-  int n = 0;
-  for (int r = lane; r < d.rows; r += 32) n += (c[r] != 0.0) ? 1 : 0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
-  if (lane == 0) d.counts[col] = n;
-}
-
-// one warp per column: ordered compaction (row indices strictly increasing, as toSparse produces them)
-__global__ void __launch_bounds__(256) csc_fill_kernel(const CscDesc* __restrict__ descs) {
-  const CscDesc d = descs[blockIdx.y];
-  const int col = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (col >= d.cols) return;
-  const double* c = d.dense + static_cast<size_t>(d.rows) * col;
-  int base = d.colPtrs[col];
-  for (int r0 = 0; r0 < d.rows; r0 += 32) {
-    const int r = r0 + lane;
-    const double v = r < d.rows ? c[r] : 0.0;
-    const bool nz = (r < d.rows) && (v != 0.0);
-    const unsigned m = __ballot_sync(0xffffffffu, nz);
-    if (nz) {
-      const int pos = base + __popc(m & ((1u << lane) - 1));
-      d.rowIndices[pos] = r;
-      d.values[pos] = v;
-    }
-    base += __popc(m);
   }
 }
 
@@ -613,24 +577,6 @@ cudaError_t launch_spmm(const int32_t* ptrs, const int32_t* idx, const double* v
     if (k <= 0) return cudaSuccess;
     dim3 grid((k + 7) / 8, n);
     spmm_csc_kernel<<<grid, 256, 0, stream>>>(ptrs, idx, vals, B, bT, C, m, k, n);
-  }
-  return cudaGetLastError();
-}
-
-cudaError_t launch_csc_count(const CscDesc* d_descs, int nblocks, int max_cols, cudaStream_t stream) {
-  if (nblocks <= 0 || max_cols <= 0) return cudaSuccess;
-  for (int off = 0; off < nblocks; off += 65535) {
-    const int nb = nblocks - off < 65535 ? nblocks - off : 65535;
-    csc_count_kernel<<<dim3((max_cols + 7) / 8, nb), 256, 0, stream>>>(d_descs + off);
-  }
-  return cudaGetLastError();
-}
-
-cudaError_t launch_csc_fill(const CscDesc* d_descs, int nblocks, int max_cols, cudaStream_t stream) {
-  if (nblocks <= 0 || max_cols <= 0) return cudaSuccess;
-  for (int off = 0; off < nblocks; off += 65535) {
-    const int nb = nblocks - off < 65535 ? nblocks - off : 65535;
-    csc_fill_kernel<<<dim3((max_cols + 7) / 8, nb), 256, 0, stream>>>(d_descs + off);
   }
   return cudaGetLastError();
 }

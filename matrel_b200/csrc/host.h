@@ -334,13 +334,4 @@ struct Slab {
   }
 };
 
-// ---- dense window -> CSC compaction (DenseMatrix.toSparse, MLMatrix.scala:392-420), batched (abi_core.cpp)
-struct DenseWin {
-  const double* p;  // column-major rows x cols
-  int32_t rows, cols;
-};
-std::vector<std::vector<int32_t>> column_counts(mr_context* ctx, const std::vector<DenseWin>& wins);
-int64_t total_count(const std::vector<int32_t>& counts);
-std::vector<Block> compact_csc(mr_context* ctx, const std::vector<DenseWin>& wins, const std::vector<std::vector<int32_t>>& counts);
-
 }  // namespace mrhost

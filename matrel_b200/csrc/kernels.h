@@ -134,7 +134,8 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
 // ---- element-wise / layout kernels (HBM-bound), batched over blocks ---------------------------------
 enum EwOp { EW_ADD = 0, EW_MUL = 1, EW_DIV = 2, EW_RANK1 = 3, EW_RANK1_COMPAT = 4, EW_COPY = 5 };
 
-// C (column-major rows x cols) = f(A(r,c), B(r,c)); A, B dense with their own isTransposed flag.
+// C (column-major rows x cols) = f(A(r,c), B(r,c)); A, B dense with their own isTransposed flag.  For EW_ADD/MUL/DIV a null A or
+// B is an absent operand: 0.0 everywhere (the unstored positions of a sparse operand, see launch_sparse_ew_scatter).
 //   EW_ADD/MUL/DIV : LocalMatrix.addDense / elementWiseOpDenseDense (LocalMatrix.scala:56-63,493-505)
 //   EW_COPY        : C = A  (DenseMatrix.toArray, MLMatrix.scala:55-61)            (B unused)
 //   EW_RANK1       : C = A + x y^T with x = B (rows), y = Y (cols)                 (intended rankOneAdd)
@@ -168,18 +169,56 @@ cudaError_t launch_sparse_to_dense(const int32_t* ptrs, const int32_t* idx, cons
 cudaError_t launch_spmm(const int32_t* ptrs, const int32_t* idx, const double* vals, bool sT,
                         const double* B, bool bT, double* C, int m, int k, int n, bool accumulate,
                         cudaStream_t stream);
-// DenseMatrix.toSparse (MLMatrix.scala:353-374) on the device, batched: (1) per-column count of v != 0.0 (NaN counts,
-// as in the reference's `arr(i) != 0`), (2) ordered per-column compaction into CSC given the column pointers.
-struct CscDesc {
-  const double* dense;   // column-major rows x cols
-  int32_t rows, cols;
-  int32_t* counts;       // [cols] out (pass 1)
-  const int32_t* colPtrs;  // [cols + 1] in (pass 2)
-  int32_t* rowIndices;   // out (pass 2)
-  double* values;        // out (pass 2)
+// ---- element-wise joins with a sparse side, on the stored entries (sparse_ew.cu, DESIGN section 4.5.3) ----------------------
+// sparse (+) sparse: one pair per output block, in a CSC frame (a CSR operand as its launch_sptrans CSC arrays).  How an operand's
+// stored entries of one position make its value:
+enum SpEwMode {
+  SPEW_SUM = 0,    // 0.0 + v1 + v2 + ... in storage order (both operands CSC: addSparseSparseNative / elementWiseOpSparseSparseNative)
+  SPEW_LAST = 1,   // the last stored v (toArray of a CSC operand when the other one is CSR)
+  SPEW_FIRST = 2,  // the first v of an ascending line with repeats adjacent (toArray of a CSR operand, repeats reversed by sptrans)
 };
-cudaError_t launch_csc_count(const CscDesc* d_descs, int nblocks, int max_cols, cudaStream_t stream);
-cudaError_t launch_csc_fill(const CscDesc* d_descs, int nblocks, int max_cols, cudaStream_t stream);
+struct SpEwPair {
+  const int32_t* ap;      // A: column pointers (cols + 1), row indices, values
+  const int32_t* ai;
+  const double* av;
+  const int32_t* bp;      // B: the same
+  const int32_t* bi;
+  const double* bv;
+  int32_t rows, cols;
+  uint8_t amode, bmode;   // SpEwMode
+  uint8_t native;         // both operands CSC: add sums A's and B's entries in one running sum; a dense outcome has +0.0 for -0.0
+  uint8_t pad;
+  int32_t* colcnt;        // count pass: [cols] kept entries of each column
+  unsigned long long* total;  // count pass: kept entries of the pair (pre-zeroed)
+  const int32_t* optr;    // fill pass, sparse outcome: column pointers (scanned from colcnt), row indices, values
+  int32_t* oidx;
+  double* oval;
+  double* dense;          // fill pass, dense outcome: column-major rows x cols, every element written (nullptr: sparse outcome)
+};
+struct SpEwLaunchShape {
+  bool acc_in_smem;       // per-warp column accumulators in shared memory, else in the caller's scratch (scratch_bytes)
+  size_t smem_bytes;
+  int max_ctas;           // persistent grid
+  size_t scratch_bytes;
+};
+constexpr int kSpEwMaxSmem = 200 * 1024;
+SpEwLaunchShape sparse_ew_shape(int max_rows);
+// op: EW_ADD / EW_MUL / EW_DIV.  fill = false: the count pass (colcnt, total); fill = true: the entries.  Every pair's rows <= max_rows.
+cudaError_t launch_sparse_ew(int op, bool fill, const SpEwPair* d_pairs, int npairs, int max_rows, int max_cols, void* d_scratch,
+                             const SpEwLaunchShape& s, cudaStream_t stream);
+// dense (+) sparse: C = op(D, S) (op(S, D) when sparse_left) at the stored positions of S, the last stored value of a position;
+// the rest of C (op with an absent operand) is written before by launch_ew_batched
+struct DsEwDesc {
+  const int32_t* ptr;     // S: CSC, or CSR when sT
+  const int32_t* idx;
+  const double* val;
+  const double* D;        // rows x cols, row-major when dT
+  double* C;              // rows x cols, column-major
+  int32_t rows, cols;
+  uint8_t sT, dT, sparse_left;
+  uint8_t pad[5];
+};
+cudaError_t launch_sparse_ew_scatter(int op, const DsEwDesc* d_descs, int ndescs, int max_lines, cudaStream_t stream);
 
 // Fused block-row SpMM: for every output block, C (col-major m x n) (+)= sum over its (CSR sparse A(i,k), dense B(k,j)) pairs.
 // One CTA = 8 output columns of one output block: the B column chunk and the C chunk live in shared memory, the K loop
