@@ -407,6 +407,8 @@ typedef struct mr_stats {
   int64_t dspmm_products;   /* sum over those pairs of stored entries of the sparse block x rows of the dense block */
   int64_t ew_sparse_pairs;  /* block pairs of the most recent element-wise join (add / multiply / divide element) with a sparse side */
   int64_t ew_sparse_entries; /* stored entries of the sparse blocks those pairs read */
+  int64_t agg_sparse_blocks; /* sparse blocks the most recent rowSum / colSum / trace / project / selection read on their stored entries */
+  int64_t agg_sparse_entries; /* stored entries of those blocks */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

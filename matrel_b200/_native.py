@@ -81,6 +81,8 @@ class mr_stats(C.Structure):
         ("dspmm_products", C.c_int64),
         ("ew_sparse_pairs", C.c_int64),
         ("ew_sparse_entries", C.c_int64),
+        ("agg_sparse_blocks", C.c_int64),
+        ("agg_sparse_entries", C.c_int64),
     ]
 
 

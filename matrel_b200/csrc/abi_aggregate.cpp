@@ -51,13 +51,22 @@ static mr_status aggregate_operator(int op, mr_matrix* a, int64_t nrows, int64_t
       r->blocks[kv.first] = op == AGG_ROW_SUM ? dense_block(kv.second, 1, s) : op == AGG_COL_SUM ? dense_block(1, kv.second, s)
                                                                                                   : dense_block(1, 1, s);
     }
+    // dense blocks: one batched launch that adds into the zeroed outputs; sparse blocks (not for sum, which adds the stored
+    // values of both kinds): per-block partials on their stored entries, combined per output in ascending block index
     std::vector<AggDesc> descs;
-    std::vector<Block> keep;
-    keep.reserve(a->blocks.size() + 1);
+    std::set<std::pair<int32_t, int32_t>> has_dense;
+    std::map<std::pair<int32_t, int32_t>, std::vector<const Block*>> sparse_of;
+    if (op != AGG_SUM) {
+      ctx->stats.agg_sparse_blocks = 0;
+      ctx->stats.agg_sparse_entries = 0;
+    }
     int max_r = 1, max_c = 1;
     for (auto& kv : a->blocks) {
       const Block& b = kv.second;
       if (op == AGG_TRACE && kv.first.first != kv.first.second) continue;
+      const std::pair<int32_t, int32_t> key = op == AGG_ROW_SUM ? std::make_pair(kv.first.first, 0)
+                                              : op == AGG_COL_SUM ? std::make_pair(0, kv.first.second)
+                                                                  : std::make_pair(0, 0);
       AggDesc d{};
       if (op == AGG_SUM) {  // values.sum over the STORED values, dense or sparse (:381-384)
         d.v = b.values.ptr<double>();
@@ -65,20 +74,19 @@ static mr_status aggregate_operator(int op, mr_matrix* a, int64_t nrows, int64_t
         d.cols = 1;
         d.isT = 0;
         if (b.valuesLen == 0) continue;
+      } else if (!b.dense()) {
+        ctx->stats.agg_sparse_blocks += 1;
+        ctx->stats.agg_sparse_entries += b.valuesLen;
+        if (b.valuesLen > 0) sparse_of[key].push_back(&b);  // an empty block adds nothing to its zeroed output
+        continue;
       } else {
-        const Block* src = &b;
-        if (!b.dense()) {
-          keep.push_back(densify(ctx, b));
-          src = &keep.back();
-        }
-        d.v = src->values.ptr<double>();
-        d.rows = src->numRows;
-        d.cols = src->numCols;
-        d.isT = src->isT;
+        d.v = b.values.ptr<double>();
+        d.rows = b.numRows;
+        d.cols = b.numCols;
+        d.isT = b.isT;
       }
-      d.out = out_ptr[op == AGG_ROW_SUM ? std::make_pair(kv.first.first, 0)
-                      : op == AGG_COL_SUM ? std::make_pair(0, kv.first.second)
-                                          : std::make_pair(0, 0)];
+      d.out = out_ptr[key];
+      has_dense.insert(key);
       max_r = std::max(max_r, d.rows);
       max_c = std::max(max_c, d.cols);
       descs.push_back(d);
@@ -86,6 +94,42 @@ static mr_status aggregate_operator(int op, mr_matrix* a, int64_t nrows, int64_t
     if (!descs.empty()) {
       Buf dd = upload(ctx, descs);
       CUDA_CHECK(launch_aggregate(op, static_cast<const AggDesc*>(dd->p), static_cast<int>(descs.size()), max_r, max_c, ctx->stream));
+      note_launch(ctx);
+    }
+    if (!sparse_of.empty()) {
+      size_t bytes = 0;
+      for (auto& kv : sparse_of) bytes += align_up(kv.second.size() * static_cast<size_t>(out_len[kv.first]) * sizeof(double));
+      Slab scratch(ctx, bytes);  // the partials, nparts x len per output
+      std::vector<SpAggDesc> sd;
+      std::vector<SpAggOut> so;
+      int max_lines = 1, max_across = 0, max_len = 1;
+      for (auto& kv : sparse_of) {
+        const int32_t len = out_len[kv.first];
+        const std::vector<const Block*>& parts = kv.second;
+        Span sp = scratch.take(parts.size() * static_cast<size_t>(len) * sizeof(double));
+        so.push_back(SpAggOut{out_ptr[kv.first], sp.ptr<double>(), len, static_cast<int32_t>(parts.size()),
+                              has_dense.count(kv.first) ? 1 : 0, 0});
+        max_len = std::max(max_len, len);
+        for (size_t i = 0; i < parts.size(); ++i) {
+          const Block& b = *parts[i];
+          SpAggDesc d{};
+          d.ptr = b.colPtrs.ptr<int32_t>();
+          d.idx = b.rowIndices.ptr<int32_t>();
+          d.val = b.values.ptr<double>();
+          d.part = sp.ptr<double>() + i * static_cast<size_t>(len);
+          d.nlines = b.isT ? b.numRows : b.numCols;
+          d.len = len;
+          d.mode = op == AGG_TRACE ? SPAGG_DIAG : (op == AGG_ROW_SUM) == b.isT ? SPAGG_ALONG : SPAGG_ACROSS;
+          if (d.mode == SPAGG_ACROSS) max_across = std::max(max_across, len);
+          max_lines = std::max(max_lines, d.nlines);
+          sd.push_back(d);
+        }
+      }
+      Buf d_sd = upload(ctx, sd), d_so = upload(ctx, so);
+      CUDA_CHECK(launch_sparse_agg(static_cast<const SpAggDesc*>(d_sd->p), static_cast<int>(sd.size()), max_lines, max_across,
+                                   ctx->stream));
+      note_launch(ctx);
+      CUDA_CHECK(launch_sparse_agg_combine(static_cast<const SpAggOut*>(d_so->p), static_cast<int>(so.size()), max_len, ctx->stream));
       note_launch(ctx);
     }
     *out = r.release();
@@ -107,48 +151,86 @@ static mr_status slice_operator(mr_matrix* a, int32_t blkSize, bool take_row, in
     const int32_t blkid = static_cast<int32_t>(index / blkSize), offset = static_cast<int32_t>(index % blkSize);  // :40-41
     const int32_t blkid2 = index2 >= 0 ? static_cast<int32_t>(index2 / blkSize) : -1;
     const int32_t offset2 = index2 >= 0 ? static_cast<int32_t>(index2 % blkSize) : -1;
-    std::vector<LineDesc> descs;
-    std::vector<std::pair<std::pair<int32_t, int32_t>, std::pair<int32_t, int32_t>>> outs;  // key -> (rows, cols)
-    std::vector<Block> keep;
-    keep.reserve(a->blocks.size() + 1);
+    ctx->stats.agg_sparse_blocks = 0;
+    ctx->stats.agg_sparse_entries = 0;
+    std::vector<LineDesc> descs;      // dense blocks
+    std::vector<SpSliceDesc> sdescs;  // sparse blocks, on their stored entries
+    struct Out {
+      std::pair<int32_t, int32_t> key;
+      int32_t rows, cols;
+      bool sparse;
+      size_t at;  // index into descs / sdescs
+    };
+    std::vector<Out> outs;
     size_t total = 0;
-    int max_len = 1;
+    int max_len = 1, max_slen = 1;
     for (auto& kv : a->blocks) {
       const int32_t rid = kv.first.first, cid = kv.first.second;
       if ((take_row ? rid : cid) != blkid) continue;                       // filter(tuple => tuple._1 == rowblkID), :48
       if (index2 >= 0 && (take_row ? cid : rid) != blkid2) continue;
-      const Block* src = &kv.second;
-      if (!src->dense()) {
-        keep.push_back(densify(ctx, *src));
-        src = &keep.back();
+      const Block& b = kv.second;
+      if (offset >= (take_row ? b.numRows : b.numCols)) continue;
+      if (index2 >= 0 && offset2 >= (take_row ? b.numCols : b.numRows)) continue;
+      const int32_t len = index2 >= 0 ? 1 : (take_row ? b.numCols : b.numRows);
+      Out o{index2 >= 0 ? std::make_pair(0, 0) : take_row ? std::make_pair(0, cid) : std::make_pair(rid, 0),
+            index2 >= 0 ? 1 : take_row ? 1 : len, index2 >= 0 ? 1 : take_row ? len : 1, !b.dense(), 0};
+      if (b.dense()) {
+        LineDesc d{};
+        d.v = b.values.ptr<double>();
+        d.rows = b.numRows;
+        d.cols = b.numCols;
+        d.offset = offset;
+        d.offset2 = offset2;
+        d.len = len;
+        d.isT = b.isT;
+        d.take_row = take_row;
+        o.at = descs.size();
+        descs.push_back(d);
+        max_len = std::max(max_len, len);
+      } else {
+        // the block's lines are its columns (CSC) or rows (CSR): a row of a CSR block or a column of a CSC one is one line; the
+        // other way, and an entry, are one index searched in each of the lines
+        SpSliceDesc d{};
+        d.ptr = b.colPtrs.ptr<int32_t>();
+        d.idx = b.rowIndices.ptr<int32_t>();
+        d.val = b.values.ptr<double>();
+        d.len = len;
+        if (index2 >= 0) {
+          d.line = b.isT ? offset : offset2;
+          d.target = b.isT ? offset2 : offset;
+        } else if (take_row == b.isT) {
+          d.line = offset;
+          d.target = -1;
+        } else {
+          d.line = 0;
+          d.target = offset;
+        }
+        o.at = sdescs.size();
+        sdescs.push_back(d);
+        max_slen = std::max(max_slen, len);
+        ctx->stats.agg_sparse_blocks += 1;
+        ctx->stats.agg_sparse_entries += b.valuesLen;
       }
-      if (offset >= (take_row ? src->numRows : src->numCols)) continue;
-      if (index2 >= 0 && offset2 >= (take_row ? src->numCols : src->numRows)) continue;
-      LineDesc d{};
-      d.v = src->values.ptr<double>();
-      d.rows = src->numRows;
-      d.cols = src->numCols;
-      d.offset = offset;
-      d.offset2 = offset2;
-      d.len = index2 >= 0 ? 1 : (take_row ? src->numCols : src->numRows);
-      d.isT = src->isT;
-      d.take_row = take_row;
-      descs.push_back(d);
-      if (index2 >= 0) outs.push_back({{0, 0}, {1, 1}});
-      else if (take_row) outs.push_back({{0, cid}, {1, d.len}});
-      else outs.push_back({{rid, 0}, {d.len, 1}});
-      total += align_up(static_cast<size_t>(d.len) * sizeof(double));
-      max_len = std::max(max_len, d.len);
+      outs.push_back(o);
+      total += align_up(static_cast<size_t>(len) * sizeof(double));
+    }
+    if (!outs.empty()) {
+      Slab slab(ctx, total);
+      for (const Out& o : outs) {
+        Span sp = slab.take(static_cast<size_t>(o.rows) * o.cols * sizeof(double));
+        if (o.sparse) sdescs[o.at].out = sp.ptr<double>();
+        else descs[o.at].out = sp.ptr<double>();
+        r->blocks[o.key] = dense_block(o.rows, o.cols, sp);
+      }
     }
     if (!descs.empty()) {
-      Slab slab(ctx, total);
-      for (size_t i = 0; i < descs.size(); ++i) {
-        Span sp = slab.take(static_cast<size_t>(descs[i].len) * sizeof(double));
-        descs[i].out = sp.ptr<double>();
-        r->blocks[outs[i].first] = dense_block(outs[i].second.first, outs[i].second.second, sp);
-      }
       Buf dd = upload(ctx, descs);
       CUDA_CHECK(launch_extract_lines(static_cast<const LineDesc*>(dd->p), static_cast<int>(descs.size()), max_len, ctx->stream));
+      note_launch(ctx);
+    }
+    if (!sdescs.empty()) {
+      Buf dd = upload(ctx, sdescs);
+      CUDA_CHECK(launch_sparse_slice(static_cast<const SpSliceDesc*>(dd->p), static_cast<int>(sdescs.size()), max_slen, ctx->stream));
       note_launch(ctx);
     }
     *out = r.release();

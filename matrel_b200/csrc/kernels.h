@@ -337,7 +337,7 @@ cudaError_t launch_spmm2(const Spmm2Item* d_items, int nitems, const Spmm2Out* d
 // the cross-block reduceByKey(LocalMatrix.add) is fused in: every block adds straight into its output vector / scalar
 // (fp64 atomics; the reference's reduce order is arbitrary as well).  Outputs must be zeroed before the launch.
 struct AggDesc {
-  const double* v;        // dense values (sparse blocks are densified by the caller)
+  const double* v;        // dense values (sparse blocks go to launch_sparse_agg)
   int32_t rows, cols;     // logical dims
   uint8_t isT;
   uint8_t pad[7];
@@ -359,6 +359,47 @@ struct LineDesc {
   double* out;
 };
 cudaError_t launch_extract_lines(const LineDesc* d_descs, int nblocks, int max_len, cudaStream_t stream);
+
+// ---- aggregates and slicing of sparse blocks on their stored entries (sparse_agg.cu, DESIGN section 4.5.4) -----------------------
+// A block's lines are the columns of a CSC block and the rows of a CSR one (colPtrs, rowIndices, values as stored).
+enum SpAggMode {
+  SPAGG_ALONG = 0,   // the output index is the line (colSum of CSC, rowSum of CSR): one lane per line
+  SPAGG_ACROSS = 1,  // the output index is the stored index (rowSum of CSC, colSum of CSR): one warp per block
+  SPAGG_DIAG = 2,    // trace: the entries whose index equals their line's, one scalar per block
+};
+struct SpAggDesc {
+  const int32_t* ptr;     // nlines + 1
+  const int32_t* idx;
+  const double* val;
+  double* part;           // out: the block's partial, len doubles, every element written
+  int32_t nlines, len;    // len: output length (rows for rowSum, columns for colSum, 1 for trace)
+  int32_t mode;           // SpAggMode
+  int32_t pad;
+};
+// One output vector and the partials of its sparse blocks, in ascending block index
+struct SpAggOut {
+  double* out;
+  const double* part;     // nparts x len, consecutive
+  int32_t len, nparts;
+  int32_t accumulate;     // 1: the line also has dense blocks, the total is added with an atomic; 0: stored
+  int32_t pad;
+};
+constexpr int kSpAggSmemLen = 2048;  // longest SPAGG_ACROSS output a warp accumulates in shared memory; longer ones in `part`
+// max_nlines: the most lines of any block; max_across_len: the longest SPAGG_ACROSS output (0: none)
+cudaError_t launch_sparse_agg(const SpAggDesc* d_descs, int ndescs, int max_nlines, int max_across_len, cudaStream_t stream);
+cudaError_t launch_sparse_agg_combine(const SpAggOut* d_outs, int nouts, int max_len, cudaStream_t stream);
+// project / selection: out[0, len) of one sparse block, the last stored entry of a position or 0.0 (every element written)
+struct SpSliceDesc {
+  const int32_t* ptr;
+  const int32_t* idx;
+  const double* val;
+  double* out;
+  int32_t len;
+  int32_t line;           // target < 0: the line copied into out; else the first of the len lines searched (out[l - line])
+  int32_t target;         // the index searched in each line, -1 = along one line
+  int32_t pad;
+};
+cudaError_t launch_sparse_slice(const SpSliceDesc* d_descs, int ndescs, int max_len, cudaStream_t stream);
 
 // Small table upload that does NOT go through the copy engines: an SM-driven copy from mapped pinned host memory.  The
 // descriptor tables of an operator must not queue behind gigabytes of block ingest on the H2D engine.
