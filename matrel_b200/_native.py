@@ -83,6 +83,8 @@ class mr_stats(C.Structure):
         ("ew_sparse_entries", C.c_int64),
         ("agg_sparse_blocks", C.c_int64),
         ("agg_sparse_entries", C.c_int64),
+        ("mv_pairs", C.c_int64),
+        ("mv_sparse_entries", C.c_int64),
     ]
 
 

@@ -31,6 +31,7 @@ struct OutPlan {
     size_t pos;  // its place in `gemm` had it been densified
   };
   std::vector<Cand> cand;                                // dense x sparse pairs that may take the route (decided by resolve)
+  std::vector<GemmSrc> mv;                               // the pairs of a matrix x vector product (run_matvec), ascending k
 };
 
 // How LocalMatrix.matrixMultiplication computes one partial product a x b (LocalMatrix.scala:889-914)
@@ -59,6 +60,7 @@ bool dspmm_candidate(const Block& a, const Block& b) {
 
 struct MultiplyPlanner {
   mr_context* ctx;
+  bool mv = false;           // the product takes the matrix x vector route: pairs are kept as they are, nothing is densified
   std::deque<Block> temps;   // densified sparse operands kept alive until the launches are enqueued (deque: the
                              // plans hold pointers to these blocks, so growth must not move them)
   std::map<const Block*, size_t> densified;
@@ -88,6 +90,10 @@ struct MultiplyPlanner {
       MR_REQUIRE(o.n == b.numCols, MR_EDIM,
                  "Matrix A and B must have the same number of cols. But found A.numCols = %d, B.numCols = %d", o.n,
                  b.numCols);
+    }
+    if (mv) {
+      o.mv.push_back(GemmSrc{&a, &b, k});
+      return;
     }
     const int kind = pair_kind(a, b);
     if (kind == PAIR_GEMM && dspmm_candidate(a, b)) {
@@ -1067,9 +1073,124 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
   note_launch(ctx);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Matrix x vector products (DESIGN section 4.5.5): C = A x (rightColNum == 1) or C = x A (leftRowNum == 1) whose vector side is all
+// dense, over matrix blocks of any kind, computed by matvec.cu as C = M x with M = A or A^T.  The pairs whose terms of an output are
+// scattered over the stored lines (CSC blocks of A x, CSR blocks of x A) and the x A pairs of CSC blocks get their partials from
+// the pre-pass; everything else, and the sum over k, is ONE launch.  No host synchronisation.
+// ------------------------------------------------------------------------------------------------
+int matvec_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, const mr_matrix* right,
+                 int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
+  auto all_dense = [](const mr_matrix* m) {
+    for (auto& kv : m->blocks)
+      if (!kv.second.dense()) return false;
+    return true;
+  };
+  int side = MV_NONE;
+  if (rightColNum == 1 && all_dense(right)) side = MV_AX;
+  else if (leftRowNum == 1 && all_dense(left)) side = MV_XA;
+  if (side == MV_NONE || ctx->gemm_algo == 0) return side;
+  // gemm_algo 1-4 request an engine for the dense x dense pairs: a product with one keeps the engines
+  const mr_matrix* mat = side == MV_AX ? left : right;
+  const mr_matrix* vec = side == MV_AX ? right : left;
+  const bool outer = ceil_div(leftColNum, blkSize) == 1 && ceil_div(rightRowNum, blkSize) == 1;  // every block meets every block
+  std::set<int32_t> ks;
+  for (auto& kv : vec->blocks) ks.insert(side == MV_AX ? kv.first.first : kv.first.second);
+  for (auto& kv : mat->blocks)
+    if (kv.second.dense() && (outer ? !ks.empty() : ks.count(side == MV_AX ? kv.first.second : kv.first.first) != 0)) return MV_NONE;
+  return side;
+}
+
+void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, bool xa) {
+  std::vector<MvOut> outs;
+  std::vector<MvPair> pairs;
+  std::vector<MvItem> items;
+  std::vector<MvPartDesc> parts;
+  std::vector<size_t> part_pair, part_off;  // per pre-pass partial: its pair, its offset (elements) in the scratch
+  size_t part_elems = 0;
+  int max_nlines = 0, max_across = 0;
+  for (size_t i = 0; i < plans.size(); ++i) {
+    const OutPlan& o = plans[i];
+    if (o.mv.empty() || o.m <= 0 || o.n <= 0) continue;
+    const int32_t len = xa ? o.n : o.m;
+    MvOut mo{};
+    mo.C = cptr[i];
+    mo.len = len;
+    mo.pair_begin = static_cast<int32_t>(pairs.size());
+    mo.pair_count = static_cast<int32_t>(o.mv.size());
+    for (const GemmSrc& g : o.mv) {
+      const Block& a = xa ? *g.b : *g.a;  // the matrix block
+      const Block& x = xa ? *g.a : *g.b;  // the vector block: kdim contiguous doubles in either layout
+      wait_ready(ctx, a);
+      wait_ready(ctx, x);
+      MvPair p{};
+      p.x = x.values.ptr<double>();
+      p.kdim = xa ? a.numRows : a.numCols;
+      ctx->stats.mv_pairs += 1;
+      if (a.dense()) {
+        p.A = a.values.ptr<double>();
+        // M(i, c) = A(i, c) for A x, A(c, i) for x A; column-major A(r, c) at r + c numRows, row-major at r numCols + c
+        const int64_t rs = a.isT ? a.numCols : 1, cs = a.isT ? 1 : a.numRows;
+        p.si = xa ? cs : rs;
+        p.sc = xa ? rs : cs;
+        p.kind = p.sc == 1 ? MV_DENSE_KCONT : MV_DENSE_ICONT;
+      } else {
+        ctx->stats.mv_sparse_entries += a.valuesLen;
+        const bool csr = a.isT;
+        if (!xa && csr) {
+          p.kind = MV_CSR;
+          p.ptr = a.colPtrs.ptr<int32_t>();
+          p.idx = a.rowIndices.ptr<int32_t>();
+          p.val = a.values.ptr<double>();
+        } else {
+          MvPartDesc d{};
+          d.ptr = a.colPtrs.ptr<int32_t>();
+          d.idx = a.rowIndices.ptr<int32_t>();
+          d.val = a.values.ptr<double>();
+          d.x = p.x;
+          d.nlines = csr ? a.numRows : a.numCols;
+          d.len = len;
+          d.xlen = p.kdim;
+          d.mode = (xa && !csr) ? MV_ALONG : MV_ACROSS;
+          d.image = xa ? 1 : 0;
+          max_nlines = std::max(max_nlines, d.mode == MV_ALONG ? d.nlines : 1);
+          if (d.mode == MV_ACROSS) max_across = std::max(max_across, len);
+          p.kind = MV_PART;
+          part_pair.push_back(pairs.size());
+          part_off.push_back(part_elems);
+          part_elems += align_up(static_cast<size_t>(len) * sizeof(double)) / sizeof(double);
+          parts.push_back(d);
+        }
+      }
+      pairs.push_back(p);
+    }
+    const int32_t oi = static_cast<int32_t>(outs.size());
+    outs.push_back(mo);
+    for (int32_t t = 0; t * kMvTile < len; ++t) items.push_back(MvItem{oi, t});
+  }
+  if (items.empty()) return;
+  Buf scratch;
+  if (!parts.empty()) {  // the partials: at most one output block's length per pair
+    scratch = std::make_shared<DevBuf>(ctx, part_elems * sizeof(double));
+    double* base = static_cast<double*>(scratch->p);
+    for (size_t t = 0; t < parts.size(); ++t) {
+      parts[t].part = base + part_off[t];
+      pairs[part_pair[t]].part = base + part_off[t];
+    }
+    Buf d_parts = upload(ctx, parts);
+    CUDA_CHECK(launch_matvec_parts(static_cast<const MvPartDesc*>(d_parts->p), static_cast<int>(parts.size()), max_nlines, max_across,
+                                   ctx->stream));
+    note_launch(ctx);
+  }
+  Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_items = upload(ctx, items);
+  CUDA_CHECK(launch_matvec(static_cast<const MvOut*>(d_outs->p), static_cast<const MvPair*>(d_pairs->p),
+                           static_cast<const MvItem*>(d_items->p), static_cast<int>(items.size()), ctx->stream));
+  note_launch(ctx);
+}
+
 void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner& planner, int32_t blkSize,
                   mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows,
-                  const MultiplyDecisions* decisions) {
+                  const MultiplyDecisions* decisions, int mv_side) {
   const ShardInfo* out_shard = result->shard.get();
   // Low-density sparse x sparse pairs: next to any dense partial the block sum is dense whatever the partial's own format
   // (LocalMatrix.add), so there they are ordinary sparse x dense products of the densified right operand; an output block
@@ -1122,6 +1243,10 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       cptr[i] = s.ptr<double>();
       result->blocks[{o.rid, o.cid}] = dense_block(o.m, o.n, s, false);  // product is never transposed (MLMatrix.scala:101)
     }
+  }
+  if (mv_side != MV_NONE) {
+    run_matvec(ctx, plans, cptr, mv_side == MV_XA);
+    return;
   }
 
   // ---- fused GEMM launch over every output block that has dense pairs
@@ -1568,6 +1693,9 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
   for (auto& kv : right->blocks)
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
   MultiplyPlanner planner{ctx};
+  const int mv_side = decisions ? decisions->mv
+                                : matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
+  planner.mv = mv_side != MV_NONE;
   std::vector<OutPlan> plans;
   const int64_t leftColBlkNum = ceil_div(leftColNum, blkSize);    // MatfastExecution.scala:712
   const int64_t rightRowBlkNum = ceil_div(rightRowNum, blkSize);  // :713
@@ -1619,14 +1747,17 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
   std::unique_ptr<mr_matrix> result(out_layout ? new_sharded(ctx, *out_layout, false, false) : new_matrix(ctx));
   if (out_layout) result->blocks.clear();  // only the blocks the product has are present (join semantics); absent ones stay absent
   run_multiply(ctx, plans, planner, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, leftColBlkNum == 1 && rightRowBlkNum == 1,
-               out_windows, decisions);
+               out_windows, decisions, mv_side);
   return result.release();
 }
 
 // The output blocks of left x right and their partial products, walked exactly as multiply_impl builds its plans (join on k in
 // ascending k, or the outer-product path with the last duplicate winning), but from metadata: no block is touched.
-MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, const mr_matrix* right, int64_t leftColNum,
-                                     int64_t rightRowNum, int32_t blkSize) {
+MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum,
+                                     const mr_matrix* right, int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
+  MultiplyDecisions d;
+  d.mv = matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
+  if (d.mv != MV_NONE) return d;
   using Id = std::pair<int32_t, int32_t>;
   struct Out {
     int32_t m = 0, n = 0;
@@ -1664,7 +1795,6 @@ MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* lef
       for (auto& jb : rit->second) pair_into(outs[{l.first.first, jb.first}], l.first, l.second, {l.first.second, jb.first}, *jb.second);
     }
   }
-  MultiplyDecisions d;
   int64_t flops = 0, tiles128 = 0;
   bool mixed = false;
   for (auto& kv : outs) {
@@ -1736,6 +1866,8 @@ mr_status mr_matrix_multiply(mr_matrix* left, int64_t leftRowNum, int64_t leftCo
     ctx->stats.spgemm_products = 0;
     ctx->stats.dspmm_pairs = 0;
     ctx->stats.dspmm_products = 0;
+    ctx->stats.mv_pairs = 0;
+    ctx->stats.mv_sparse_entries = 0;
     if (left->host || right->host)  // C tile by C tile through the device, into a host-resident result (abi_stream.cpp)
       *out = multiply_streamed(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
     else

@@ -105,7 +105,7 @@ int64_t payload(const Block& b) {  // bytes of a block's arrays
 
 mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right,
                              int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
-  const MultiplyDecisions dec = multiply_decisions(ctx, left, right, leftColNum, rightRowNum, blkSize);
+  const MultiplyDecisions dec = multiply_decisions(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
   // ---- the block rows of A and block columns of B (ascending ids): a panel is a run of consecutive entries
   std::map<int32_t, size_t> row_dev, col_dev;  // device bytes per block row of A / block column of B
   std::map<int32_t, size_t> row_fp, row_dense, col_dense;  // stored and dense-image bytes of a block row of A / column of B
@@ -169,8 +169,11 @@ mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNu
   // row-major copies of the column-major dense B blocks a sparse x dense kernel reads
   // Right blocks of dense x sparse pairs that take the stored-entry route get no dense image: their prepared segments (and CSC
   // copy) instead, and their left blocks a column-major copy and non-finite sets (DESIGN section 4.5.2).
-  const size_t a_scratch = (a_sparse ? a_row_dense + a_row_fp : 0) + a_ds_max;
-  const size_t b_scratch = (a_sparse ? 1 : 0) * b_col_dense + (b_sparse ? b_col_ds_max : 0);
+  // The matrix x vector route (DESIGN section 4.5.5) makes no images: its scratch is at most one output block per pair.
+  const bool mv = dec.mv != MV_NONE;
+  const size_t a_scratch = mv ? 0 : (a_sparse ? a_row_dense + a_row_fp : 0) + a_ds_max;
+  const size_t b_scratch = mv ? 0 : (a_sparse ? 1 : 0) * b_col_dense + (b_sparse ? b_col_ds_max : 0);
+  const int64_t kblocks = ceil_div(leftColNum, blkSize);
   // ---- device budget and the tile
   const size_t budget = stream_budget(ctx);
   const size_t c_block = align_up(static_cast<size_t>(max_m) * max_n * sizeof(double));
@@ -178,7 +181,8 @@ mr_matrix* multiply_streamed(mr_context* ctx, mr_matrix* left, int64_t leftRowNu
       static_cast<int64_t>(rows.size()), static_cast<int64_t>(cols.size()), a_row, b_col, a_bytes, b_bytes, c_block, budget,
       [&](int64_t tr, int64_t tc) {
         const size_t oz2 = dec.oz2 ? oz2_scratch_for(ctx, blkSize, leftColNum, static_cast<int>(tr), static_cast<int>(tc)) : 0;
-        return oz2 + static_cast<size_t>(tr) * a_scratch + static_cast<size_t>(tc) * b_scratch;
+        const size_t mv_parts = mv ? static_cast<size_t>(tr) * tc * kblocks * c_block : 0;
+        return oz2 + mv_parts + static_cast<size_t>(tr) * a_scratch + static_cast<size_t>(tc) * b_scratch;
       });
   if (!T.ok)
     fail(MR_ENOMEM,

@@ -270,7 +270,9 @@ using OutWindowFn = std::function<Span(int32_t rid, int32_t cid)>;
 // The choices multiply_impl otherwise derives from the shape it is given.  A streamed multiply computes them once for the whole
 // product and hands them to every tile, so that each output element takes the same engine and kernel variant as in the resident
 // call: oz2 = try the Ozaki-II engine, variant = DMMA tile variant (gemm_variant still overrides it).
+enum MvSide { MV_NONE = 0, MV_AX = 1, MV_XA = 2 };  // no matrix x vector route, C = A x, C = x A (abi_multiply.cpp, run_matvec)
 struct MultiplyDecisions {
+  int mv = MV_NONE;  // the matrix x vector route (then nothing else below applies)
   bool oz2 = false;
   int variant = 0;
   // dense x sparse pairs (ids of their blocks): left and right blocks of the pairs that take the stored-entry route, and right
@@ -281,8 +283,8 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
                          int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr,
                          const MultiplyDecisions* decisions = nullptr);
 // The decisions multiply_impl would take for left x right, from block metadata only (the blocks may be host-resident).
-MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, const mr_matrix* right, int64_t leftColNum,
-                                     int64_t rightRowNum, int32_t blkSize);
+MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum,
+                                     const mr_matrix* right, int64_t rightRowNum, int64_t rightColNum, int32_t blkSize);
 // Scratch the dense x low-density sparse route allocates for one left / right block of its pairs (upper bounds).
 size_t dspmm_left_scratch(const Block& a);
 size_t dspmm_right_scratch(const Block& b);

@@ -401,6 +401,53 @@ struct SpSliceDesc {
 };
 cudaError_t launch_sparse_slice(const SpSliceDesc* d_descs, int ndescs, int max_len, cudaStream_t stream);
 
+// ---- matrix x vector products C = M x over dense, CSC and CSR blocks (matvec.cu, DESIGN section 4.5.5) ----------------------------
+// M = A for C = A x, M = A^T for C = x A.  Each output block has its pairs (k-blocks) in ascending k; x is a pair's vector block
+// (kdim contiguous doubles).
+enum MvKind {
+  MV_DENSE_ICONT = 0,  // dense, M(i, c) at A[i + c sc]
+  MV_DENSE_KCONT = 1,  // dense, M(i, c) at A[i si + c]
+  MV_CSR = 2,          // the CSR arrays of M (A x with a CSR block)
+  MV_PART = 3,         // the partial launch_matvec_parts wrote
+};
+struct MvPair {
+  const double* A;
+  const int32_t* ptr;     // MV_CSR: row pointers, column indices, values
+  const int32_t* idx;
+  const double* val;
+  const double* x;
+  const double* part;     // MV_PART: len doubles
+  int64_t si, sc;
+  int32_t kdim, kind;
+};
+struct MvOut {
+  double* C;              // len doubles (an m x 1 or 1 x n column-major block), every element written
+  int32_t len, pair_begin, pair_count, pad;
+};
+constexpr int kMvTile = 32;  // outputs per CTA
+struct MvItem {           // one CTA: outputs [tile * kMvTile, +kMvTile) of one output block
+  int32_t out, tile;
+};
+cudaError_t launch_matvec(const MvOut* d_outs, const MvPair* d_pairs, const MvItem* d_items, int nitems, cudaStream_t stream);
+enum MvPartMode {
+  MV_ALONG = 0,   // the output index is the line (x S with a CSC block): one lane per line, x indexed by the stored index
+  MV_ACROSS = 1,  // the output index is the stored index (A x with a CSC block, x S with a CSR block): one warp, x indexed by the line
+};
+struct MvPartDesc {
+  const int32_t* ptr;     // nlines + 1, as stored
+  const int32_t* idx;
+  const double* val;
+  const double* x;        // xlen doubles
+  double* part;           // out: len doubles, every element written
+  int32_t nlines, len, xlen;
+  int32_t mode;           // MvPartMode
+  int32_t image;          // 1 (x S): the dense image's terms (the last stored entry of a position; NaN where a non-finite x meets an
+                          // unstored position)
+  int32_t pad;
+};
+constexpr int kMvPartSmemLen = 2048;  // longest MV_ACROSS output a warp accumulates in shared memory; longer ones in `part`
+cudaError_t launch_matvec_parts(const MvPartDesc* d_descs, int ndescs, int max_nlines, int max_across_len, cudaStream_t stream);
+
 // Small table upload that does NOT go through the copy engines: an SM-driven copy from mapped pinned host memory.  The
 // descriptor tables of an operator must not queue behind gigabytes of block ingest on the H2D engine.
 cudaError_t launch_copy_words(void* dst, const void* src_mapped, size_t bytes, cudaStream_t stream);
