@@ -409,8 +409,9 @@ typedef struct mr_stats {
   int64_t ew_sparse_entries; /* stored entries of the sparse blocks those pairs read */
   int64_t agg_sparse_blocks; /* sparse blocks the most recent rowSum / colSum / trace / project / selection read on their stored entries */
   int64_t agg_sparse_entries; /* stored entries of those blocks */
-  int64_t mv_pairs;         /* block pairs of the most recent mr_matrix_multiply computed by the matrix x vector route (summed over the
-                               tiles of a streamed multiply) */
+  int64_t mv_pairs;         /* block pairs of the most recent mr_matrix_multiply computed by the matrix x vector / thin-matrix route
+                               (thin side of 1 to 8 dense columns or rows; a pair is a matrix block and a thin-side block, whatever
+                               its width; summed over the tiles of a streamed multiply) */
   int64_t mv_sparse_entries; /* stored entries of the sparse blocks among those pairs */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);

@@ -1074,8 +1074,8 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
 }
 
 // ------------------------------------------------------------------------------------------------
-// Matrix x vector products (DESIGN section 4.5.5): C = A x (rightColNum == 1) or C = x A (leftRowNum == 1) whose vector side is all
-// dense, over matrix blocks of any kind, computed by matvec.cu as C = M x with M = A or A^T.  The pairs whose terms of an output are
+// Matrix x thin-matrix products (DESIGN section 4.5.5): C = A X (rightColNum <= kMvMaxCols) or C = X A (leftRowNum <= kMvMaxCols)
+// whose thin side is all dense, over matrix blocks of any kind, computed by matvec.cu as C = M X with M = A or A^T.  The pairs whose terms of an output are
 // scattered over the stored lines (CSC blocks of A x, CSR blocks of x A) and the x A pairs of CSC blocks get their partials from
 // the pre-pass; everything else, and the sum over k, is ONE launch.  No host synchronisation.
 // ------------------------------------------------------------------------------------------------
@@ -1087,8 +1087,8 @@ int matvec_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNu
     return true;
   };
   int side = MV_NONE;
-  if (rightColNum == 1 && all_dense(right)) side = MV_AX;
-  else if (leftRowNum == 1 && all_dense(left)) side = MV_XA;
+  if (rightColNum >= 1 && rightColNum <= kMvMaxCols && all_dense(right)) side = MV_AX;
+  else if (leftRowNum >= 1 && leftRowNum <= kMvMaxCols && all_dense(left)) side = MV_XA;
   if (side == MV_NONE || ctx->gemm_algo == 0) return side;
   // gemm_algo 1-4 request an engine for the dense x dense pairs: a product with one keeps the engines
   const mr_matrix* mat = side == MV_AX ? left : right;
@@ -1106,23 +1106,30 @@ void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::v
   std::vector<MvPair> pairs;
   std::vector<MvItem> items;
   std::vector<MvPartDesc> parts;
+  std::vector<MvXLayout> pair_xl, part_xl;   // the X block strides of each pair / pre-pass partial
   std::vector<size_t> part_pair, part_off;  // per pre-pass partial: its pair, its offset (elements) in the scratch
   size_t part_elems = 0;
-  int max_nlines = 0, max_across = 0;
+  int max_nlines = 0, max_across = 0, max_cols = 1;
   for (size_t i = 0; i < plans.size(); ++i) {
     const OutPlan& o = plans[i];
     if (o.mv.empty() || o.m <= 0 || o.n <= 0) continue;
-    const int32_t len = xa ? o.n : o.m;
+    const int32_t len = xa ? o.n : o.m, cols = xa ? o.m : o.n;
+    max_cols = std::max(max_cols, static_cast<int>(cols));
     MvOut mo{};
     mo.C = cptr[i];
     mo.len = len;
+    mo.cols = cols;
     mo.pair_begin = static_cast<int32_t>(pairs.size());
     mo.pair_count = static_cast<int32_t>(o.mv.size());
     for (const GemmSrc& g : o.mv) {
       const Block& a = xa ? *g.b : *g.a;  // the matrix block
-      const Block& x = xa ? *g.a : *g.b;  // the vector block: kdim contiguous doubles in either layout
+      const Block& x = xa ? *g.a : *g.b;  // the thin block: kdim x cols (A X) or cols x kdim (X A), in either layout
       wait_ready(ctx, a);
       wait_ready(ctx, x);
+      // x(c, j) = X(c, j) for A X, X(j, c) for X A; the inner index c is contiguous when the block's layout runs along it
+      const int32_t ld = x.isT ? x.numCols : x.numRows;
+      const MvXLayout xl = xa == x.isT ? MvXLayout{1, ld} : MvXLayout{ld, 1};
+      pair_xl.push_back(xl);
       MvPair p{};
       p.x = x.values.ptr<double>();
       p.kdim = xa ? a.numRows : a.numCols;
@@ -1153,13 +1160,15 @@ void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::v
           d.xlen = p.kdim;
           d.mode = (xa && !csr) ? MV_ALONG : MV_ACROSS;
           d.image = xa ? 1 : 0;
+          d.cols = cols;
           max_nlines = std::max(max_nlines, d.mode == MV_ALONG ? d.nlines : 1);
           if (d.mode == MV_ACROSS) max_across = std::max(max_across, len);
           p.kind = MV_PART;
           part_pair.push_back(pairs.size());
           part_off.push_back(part_elems);
-          part_elems += align_up(static_cast<size_t>(len) * sizeof(double)) / sizeof(double);
+          part_elems += align_up(static_cast<size_t>(len) * cols * sizeof(double)) / sizeof(double);
           parts.push_back(d);
+          part_xl.push_back(xl);
         }
       }
       pairs.push_back(p);
@@ -1170,21 +1179,24 @@ void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::v
   }
   if (items.empty()) return;
   Buf scratch;
-  if (!parts.empty()) {  // the partials: at most one output block's length per pair
+  // The strides are only read above width 1
+  const auto xls = [&](const std::vector<MvXLayout>& v) { return max_cols > 1 ? upload(ctx, v) : Buf(); };
+  if (!parts.empty()) {  // the partials: at most one output block per pair
     scratch = std::make_shared<DevBuf>(ctx, part_elems * sizeof(double));
     double* base = static_cast<double*>(scratch->p);
     for (size_t t = 0; t < parts.size(); ++t) {
       parts[t].part = base + part_off[t];
       pairs[part_pair[t]].part = base + part_off[t];
     }
-    Buf d_parts = upload(ctx, parts);
+    Buf d_parts = upload(ctx, parts), d_part_xl = xls(part_xl);
     CUDA_CHECK(launch_matvec_parts(static_cast<const MvPartDesc*>(d_parts->p), static_cast<int>(parts.size()), max_nlines, max_across,
-                                   ctx->stream));
+                                   max_cols, d_part_xl ? static_cast<const MvXLayout*>(d_part_xl->p) : nullptr, ctx->stream));
     note_launch(ctx);
   }
-  Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_items = upload(ctx, items);
+  Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_items = upload(ctx, items), d_pair_xl = xls(pair_xl);
   CUDA_CHECK(launch_matvec(static_cast<const MvOut*>(d_outs->p), static_cast<const MvPair*>(d_pairs->p),
-                           static_cast<const MvItem*>(d_items->p), static_cast<int>(items.size()), ctx->stream));
+                           static_cast<const MvItem*>(d_items->p), static_cast<int>(items.size()), max_cols,
+                           d_pair_xl ? static_cast<const MvXLayout*>(d_pair_xl->p) : nullptr, xa, ctx->stream));
   note_launch(ctx);
 }
 

@@ -401,13 +401,15 @@ struct SpSliceDesc {
 };
 cudaError_t launch_sparse_slice(const SpSliceDesc* d_descs, int ndescs, int max_len, cudaStream_t stream);
 
-// ---- matrix x vector products C = M x over dense, CSC and CSR blocks (matvec.cu, DESIGN section 4.5.5) ----------------------------
-// M = A for C = A x, M = A^T for C = x A.  Each output block has its pairs (k-blocks) in ascending k; x is a pair's vector block
-// (kdim contiguous doubles).
+// ---- matrix x thin-matrix products C = M X over dense, CSC and CSR blocks (matvec.cu, DESIGN section 4.5.5) -----------------------
+// M = A for C = A X, M = A^T for C = X A.  X has cols <= kMvMaxCols columns (rows for X A), the kernels run a width W in {1, 2, 4, 8}
+// >= cols, and column j of C is computed exactly as the width-1 product M X(:, j).  Each output block has its pairs (k-blocks) in
+// ascending k; x is a pair's X block: kdim contiguous doubles at width 1, x(c, j) at x[c xl.c + j xl.j] (MvXLayout) above.
+constexpr int kMvMaxCols = 8;
 enum MvKind {
   MV_DENSE_ICONT = 0,  // dense, M(i, c) at A[i + c sc]
   MV_DENSE_KCONT = 1,  // dense, M(i, c) at A[i si + c]
-  MV_CSR = 2,          // the CSR arrays of M (A x with a CSR block)
+  MV_CSR = 2,          // the CSR arrays of M (A X with a CSR block)
   MV_PART = 3,         // the partial launch_matvec_parts wrote
 };
 struct MvPair {
@@ -416,37 +418,45 @@ struct MvPair {
   const int32_t* idx;
   const double* val;
   const double* x;
-  const double* part;     // MV_PART: len doubles
+  const double* part;     // MV_PART: column j of the partial at part[j len], len doubles each
   int64_t si, sc;
   int32_t kdim, kind;
 };
+// The strides of an X block, one per MvPair / MvPartDesc in an array of their own: the width-1 kernels read neither it nor `cols`,
+// so their code and the descriptors' sizes are those of the single-vector route.
+struct MvXLayout {
+  int32_t c, j;
+};
 struct MvOut {
-  double* C;              // len doubles (an m x 1 or 1 x n column-major block), every element written
-  int32_t len, pair_begin, pair_count, pad;
+  double* C;              // len x cols column-major (A X: (i, j) at i + j len) or cols x len (X A: (j, i) at j + i cols), every
+                          // element written
+  int32_t len, pair_begin, pair_count, cols;
 };
 constexpr int kMvTile = 32;  // outputs per CTA
 struct MvItem {           // one CTA: outputs [tile * kMvTile, +kMvTile) of one output block
   int32_t out, tile;
 };
-cudaError_t launch_matvec(const MvOut* d_outs, const MvPair* d_pairs, const MvItem* d_items, int nitems, cudaStream_t stream);
+// max_cols: the widest output block (picks W); d_xls: one MvXLayout per pair, unread (may be null) when max_cols == 1; xa: C = X A
+cudaError_t launch_matvec(const MvOut* d_outs, const MvPair* d_pairs, const MvItem* d_items, int nitems, int max_cols,
+                          const MvXLayout* d_xls, int xa, cudaStream_t stream);
 enum MvPartMode {
-  MV_ALONG = 0,   // the output index is the line (x S with a CSC block): one lane per line, x indexed by the stored index
-  MV_ACROSS = 1,  // the output index is the stored index (A x with a CSC block, x S with a CSR block): one warp, x indexed by the line
+  MV_ALONG = 0,   // the output index is the line (X S with a CSC block): one lane per line, x indexed by the stored index
+  MV_ACROSS = 1,  // the output index is the stored index (A X with a CSC block, X S with a CSR block): one warp, x indexed by the line
 };
 struct MvPartDesc {
   const int32_t* ptr;     // nlines + 1, as stored
   const int32_t* idx;
   const double* val;
-  const double* x;        // xlen doubles
-  double* part;           // out: len doubles, every element written
+  const double* x;        // X block: xlen rows (c) x cols
+  double* part;           // out: column j at part[j len], len doubles each, every element written
   int32_t nlines, len, xlen;
   int32_t mode;           // MvPartMode
-  int32_t image;          // 1 (x S): the dense image's terms (the last stored entry of a position; NaN where a non-finite x meets an
-                          // unstored position)
-  int32_t pad;
+  int32_t image;          // 1 (X S): the dense image's terms (the last stored entry of a position; NaN in column j where a non-finite
+                          // x(r, j) meets an unstored position)
+  int32_t cols;
 };
-constexpr int kMvPartSmemLen = 2048;  // longest MV_ACROSS output a warp accumulates in shared memory; longer ones in `part`
-cudaError_t launch_matvec_parts(const MvPartDesc* d_descs, int ndescs, int max_nlines, int max_across_len, cudaStream_t stream);
+cudaError_t launch_matvec_parts(const MvPartDesc* d_descs, int ndescs, int max_nlines, int max_across_len, int max_cols,
+                                const MvXLayout* d_xls, cudaStream_t stream);
 
 // Small table upload that does NOT go through the copy engines: an SM-driven copy from mapped pinned host memory.  The
 // descriptor tables of an operator must not queue behind gigabytes of block ingest on the H2D engine.
