@@ -69,9 +69,11 @@ static mr_status aggregate_operator(int op, mr_matrix* a, int64_t nrows, int64_t
                                                                   : std::make_pair(0, 0);
       AggDesc d{};
       if (op == AGG_SUM) {  // values.sum over the STORED values, dense or sparse (:381-384)
+        // a dense block may hold 2^31 values or more, so it is described by its shape; a sparse block's int32 colPtrs bound its
+        // valuesLen by INT32_MAX
         d.v = b.values.ptr<double>();
-        d.rows = static_cast<int32_t>(std::min<int64_t>(b.valuesLen, INT32_MAX));
-        d.cols = 1;
+        d.rows = b.dense() ? b.numRows : static_cast<int32_t>(b.valuesLen);
+        d.cols = b.dense() ? b.numCols : 1;
         d.isT = 0;
         if (b.valuesLen == 0) continue;
       } else if (!b.dense()) {

@@ -143,7 +143,8 @@ __global__ void __launch_bounds__(256) ew_tiled_kernel(const EwDesc* __restrict_
     const int c = c0 + ty + 8 * j;
     if (r < d.rows && c < d.cols) {
       double out;
-      if (OP == EW_RANK1) out = a[j] + d.B[r] * d.Y[c];
+      // a + (x y) with both operations rounded, as LocalMatrix.rankOneAdd: a contracted FMA would round once
+      if (OP == EW_RANK1) out = __dadd_rn(a[j], __dmul_rn(d.B[r], d.Y[c]));
       else out = ew_apply<OP>(a[j], b[j]);
       d.C[r + static_cast<size_t>(d.rows) * c] = out;
     }
@@ -163,6 +164,8 @@ __device__ __forceinline__ double map_apply(double v, double alpha) {
     if (isinf(v) && v < 0.0) return -v;             // pow(-inf, 0.5) = +inf
     return sqrt(v);
   }
+  // java.lang.Math.pow, unlike C's pow, gives NaN for pow(+-1, +-inf) and pow(1, NaN)
+  if (!isfinite(alpha) && fabs(v) == 1.0) return __longlong_as_double(0x7ff8000000000000LL);
   return pow(v, alpha);
 }
 

@@ -482,10 +482,17 @@ def addScalar(mat: MLMatrix, alpha: float) -> MLMatrix:
 
 
 def matrixPow(mat: MLMatrix, p: float) -> MLMatrix:
-    """M/matrix/LocalMatrix.scala:931-946 -- math.pow on stored values."""
+    """M/matrix/LocalMatrix.scala:931-946 -- math.pow on stored values.  math.pow is java.lang.Math.pow, which differs from C's
+    pow in one case: pow(+-1, p) is NaN for an infinite or NaN p, where C gives 1.0.  np.power(v, 0.5) is sqrt(v), which also
+    differs at -0.0 and -inf (Java: +0.0 and +inf)."""
     def f(v):
         with np.errstate(all="ignore"):
-            return np.power(v, p)
+            r = np.power(v, p)
+        if not math.isfinite(p):
+            r = np.where(np.abs(v) == 1.0, np.nan, r)
+        elif p == 0.5:
+            r = np.where((v == 0.0) | np.isneginf(v), np.abs(v), r)
+        return r
     return _map_values(mat, f)
 
 
