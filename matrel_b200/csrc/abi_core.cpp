@@ -132,6 +132,49 @@ Block densify(mr_context* ctx, const Block& s) {
   return dense_block(s.numRows, s.numCols, v, false);
 }
 
+CscLayout::CscLayout(int32_t cols, int64_t nnz) {
+  ptr = 0;
+  idx = align_up((static_cast<size_t>(cols) + 1) * sizeof(int32_t));
+  val = idx + align_up(static_cast<size_t>(nnz) * sizeof(int32_t));
+  bytes = val + align_up(static_cast<size_t>(nnz) * sizeof(double));
+}
+
+void csr_to_csc(mr_context* ctx, const std::vector<CsrToCsc>& convs) {
+  if (convs.empty()) return;
+  size_t cursors = 0;
+  for (const CsrToCsc& c : convs) cursors += static_cast<size_t>(c.cols);
+  Buf cur = std::make_shared<DevBuf>(ctx, std::max<size_t>(cursors, 1) * sizeof(int32_t));
+  CUDA_CHECK(cudaMemsetAsync(cur->p, 0, cursors * sizeof(int32_t), ctx->stream));
+  std::vector<SpTransDesc> td;
+  std::vector<ScanDesc> sd;
+  int max_nnz = 0, max_nl = 0, max_no = 0;
+  int32_t* next = static_cast<int32_t*>(cur->p);
+  for (const CsrToCsc& c : convs) {
+    const CscLayout L(c.cols, c.nnz);
+    SpTransDesc d{};
+    d.ptr = c.ptr;
+    d.idx = c.idx;
+    d.val = c.val;
+    d.nl = c.rows;
+    d.no = c.cols;
+    d.nnz = static_cast<int32_t>(c.nnz);
+    d.optr = reinterpret_cast<int32_t*>(c.out + L.ptr);
+    d.oidx = reinterpret_cast<int32_t*>(c.out + L.idx);
+    d.oval = reinterpret_cast<double*>(c.out + L.val);
+    d.cur = next;
+    next += c.cols;
+    td.push_back(d);
+    sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
+    max_nnz = std::max(max_nnz, d.nnz);
+    max_nl = std::max(max_nl, d.nl);
+    max_no = std::max(max_no, d.no);
+  }
+  Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
+  CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
+                            max_nnz, max_nl, max_no, ctx->stream));
+  note_launch(ctx, 4);
+}
+
 const char* type_name(const Block& b) { return b.dense() ? "DenseMatrix" : "SparseMatrix"; }
 
 int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }

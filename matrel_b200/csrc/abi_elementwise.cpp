@@ -77,58 +77,25 @@ struct SparsePair {
 void sparse_sparse_join(mr_context* ctx, int op, const std::vector<SparsePair>& jobs, mr_matrix* result) {
   if (jobs.empty()) return;
   const size_t np = jobs.size();
-  // ---- CSR operands through sptrans, once per block: scratch = cursors (zeroed), then the CSC arrays
-  struct Conv {
-    size_t ptr, idx, val, cur;
-  };
-  std::map<const Block*, Conv> conv;
-  size_t cur_bytes = 0, conv_bytes = 0;
+  // ---- CSR operands through sptrans, once per block
+  std::map<const Block*, size_t> conv;  // block -> offset of its CSC copy in the scratch
+  size_t conv_bytes = 0;
   for (auto& j : jobs)
     for (const Block* b : {j.a, j.b})
       if (b->isT && !conv.count(b)) {
-        Conv v{};
-        v.cur = cur_bytes;
-        cur_bytes += align_up(static_cast<size_t>(b->numCols) * sizeof(int32_t));
-        v.ptr = conv_bytes;
-        conv_bytes += align_up(static_cast<size_t>(b->numCols + 1) * sizeof(int32_t));
-        v.idx = conv_bytes;
-        conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(int32_t));
-        v.val = conv_bytes;
-        conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(double));
-        conv.emplace(b, v);
+        conv.emplace(b, conv_bytes);
+        conv_bytes += CscLayout(b->numCols, b->valuesLen).bytes;
       }
   Buf cbuf;
   if (!conv.empty()) {
-    cbuf = std::make_shared<DevBuf>(ctx, cur_bytes + conv_bytes);
-    CUDA_CHECK(cudaMemsetAsync(cbuf->p, 0, cur_bytes, ctx->stream));
-    char* base = static_cast<char*>(cbuf->p);
-    std::vector<SpTransDesc> td;
-    std::vector<ScanDesc> sd;
-    int max_nnz = 0, max_nl = 0, max_no = 0;
+    cbuf = std::make_shared<DevBuf>(ctx, conv_bytes);
+    std::vector<CsrToCsc> cv;
     for (auto& kv : conv) {
       const Block* b = kv.first;
-      const Conv& v = kv.second;
-      SpTransDesc d{};
-      d.ptr = b->colPtrs.ptr<int32_t>();
-      d.idx = b->rowIndices.ptr<int32_t>();
-      d.val = b->values.ptr<double>();
-      d.nl = b->numRows;
-      d.no = b->numCols;
-      d.nnz = static_cast<int32_t>(b->valuesLen);
-      d.optr = reinterpret_cast<int32_t*>(base + cur_bytes + v.ptr);
-      d.oidx = reinterpret_cast<int32_t*>(base + cur_bytes + v.idx);
-      d.oval = reinterpret_cast<double*>(base + cur_bytes + v.val);
-      d.cur = reinterpret_cast<int32_t*>(base + v.cur);
-      td.push_back(d);
-      sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
-      max_nnz = std::max(max_nnz, d.nnz);
-      max_nl = std::max(max_nl, d.nl);
-      max_no = std::max(max_no, d.no);
+      cv.push_back(CsrToCsc{b->colPtrs.ptr<int32_t>(), b->rowIndices.ptr<int32_t>(), b->values.ptr<double>(), b->numRows, b->numCols,
+                            b->valuesLen, static_cast<char*>(cbuf->p) + kv.second});
     }
-    Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
-    CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
-                              max_nnz, max_nl, max_no, ctx->stream));
-    note_launch(ctx, 4);
+    csr_to_csc(ctx, cv);
   }
   // ---- the pairs in the CSC frame
   size_t col_total = 0;
@@ -148,11 +115,11 @@ void sparse_sparse_join(mr_context* ctx, int op, const std::vector<SparsePair>& 
     SpEwPair& q = pairs[i];
     auto csc_of = [&](const Block* x, const int32_t*& p, const int32_t*& ix, const double*& v, uint8_t& mode) {
       if (x->isT) {
-        const Conv& cv = conv.at(x);
-        char* base = static_cast<char*>(cbuf->p) + cur_bytes;
-        p = reinterpret_cast<const int32_t*>(base + cv.ptr);
-        ix = reinterpret_cast<const int32_t*>(base + cv.idx);
-        v = reinterpret_cast<const double*>(base + cv.val);
+        const char* w = static_cast<const char*>(cbuf->p) + conv.at(x);
+        const CscLayout L(x->numCols, x->valuesLen);
+        p = reinterpret_cast<const int32_t*>(w + L.ptr);
+        ix = reinterpret_cast<const int32_t*>(w + L.idx);
+        v = reinterpret_cast<const double*>(w + L.val);
         mode = SPEW_FIRST;
       } else {
         p = x->colPtrs.ptr<int32_t>();

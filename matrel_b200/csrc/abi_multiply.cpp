@@ -10,30 +10,6 @@ namespace {
 // ------------------------------------------------------------------------------------------------
 // block product planning (LocalMatrix.matrixMultiplication, LocalMatrix.scala:889-914)
 // ------------------------------------------------------------------------------------------------
-struct GemmSrc {
-  const Block* a;
-  const Block* b;
-  int32_t k;
-};
-
-struct OutPlan {
-  int32_t rid, cid;
-  int32_t m = -1, n = -1;
-  std::vector<GemmPair> gemm;                            // dense x dense (possibly densified) pairs
-  std::vector<GemmSrc> src;                              // the blocks behind each gemm pair (+ its k-block id)
-  std::vector<std::pair<const Block*, const Block*>> spmm;  // sparse x dense pairs
-  std::vector<std::pair<const Block*, const Block*>> spsp;  // sparse x sparse, both densities <= 0.1 (ascending k)
-  std::vector<std::pair<const Block*, const Block*>> dspmm; // dense x low-density sparse on the stored entries (dspmm_route)
-  struct Cand {
-    const Block* a;
-    const Block* b;
-    int32_t k;
-    size_t pos;  // its place in `gemm` had it been densified
-  };
-  std::vector<Cand> cand;                                // dense x sparse pairs that may take the route (decided by resolve)
-  std::vector<GemmSrc> mv;                               // the pairs of a matrix x vector product (run_matvec), ascending k
-};
-
 // How LocalMatrix.matrixMultiplication computes one partial product a x b (LocalMatrix.scala:889-914)
 enum PairKind { PAIR_GEMM = 0, PAIR_SPMM = 1, PAIR_SPSP = 2 };
 int pair_kind(const Block& a, const Block& b) {
@@ -58,27 +34,58 @@ bool dspmm_candidate(const Block& a, const Block& b) {
   return b.valuesLen * 1.0 / (static_cast<double>(b.numRows) * b.numCols) <= kDspmmMaxDensity;
 }
 
-struct MultiplyPlanner {
-  mr_context* ctx;
-  bool mv = false;           // the product takes the matrix x vector route: pairs are kept as they are, nothing is densified
-  std::deque<Block> temps;   // densified sparse operands kept alive until the launches are enqueued (deque: the
-                             // plans hold pointers to these blocks, so growth must not move them)
-  std::map<const Block*, size_t> densified;
+// Where one partial product of an output block is computed
+enum Route : uint8_t {
+  ROUTE_GEMM,       // the dense engines; a sparse operand through its dense image
+  ROUTE_SPMM,       // sparse x dense (the n == 1 SpMV case is the same kernel); a sparse right operand through its dense image
+  ROUTE_SPSP,       // low-density sparse x sparse in a block made of such pairs only (run_sparse_chains)
+  ROUTE_SPSP_SPMM,  // low-density sparse x sparse next to other partials: sparse x the dense image of the right operand
+  ROUTE_DSPMM,      // dense x low-density sparse from the stored entries (run_dense_sparse)
+  ROUTE_MV,         // matrix x thin matrix (run_matvec)
+};
 
-  const Block& dense_of(const Block& b) {
-    if (b.dense()) return b;
-    auto it = densified.find(&b);
-    if (it == densified.end()) {
-      temps.push_back(densify(ctx, b));
-      it = densified.emplace(&b, temps.size() - 1).first;
-    }
-    return temps[it->second];
+struct PlanPair {
+  const Block* a;
+  const Block* b;
+  int32_t k, kb;  // the blocks are a = (rid, k) and b = (kb, cid); k == kb except in the outer product
+  Route route;
+};
+
+struct OutPlan {
+  int32_t rid, cid;
+  int32_t m = -1, n = -1;
+  std::vector<PlanPair> pairs;  // ascending k
+  bool has(Route r) const {
+    return std::any_of(pairs.begin(), pairs.end(), [r](const PlanPair& p) { return p.route == r; });
   }
+  bool only(Route r) const {
+    return std::all_of(pairs.begin(), pairs.end(), [r](const PlanPair& p) { return p.route == r; });
+  }
+  bool has_spmm() const { return has(ROUTE_SPMM) || has(ROUTE_SPSP_SPMM); }
+};
 
-  void add_pair(OutPlan& o, const Block& a, const Block& b, int32_t k) {
+// The output blocks of left x right and the route of every partial product, from block metadata only (the blocks may be
+// host-resident).  outer: the outer-product paths (MatfastExecution.scala:714-721 -> helper :175-221), every left block x every
+// right block with no reduce, the last duplicate key winning as when collected into a map (reference defect B1, DuplicateLeft
+// throws, is not reproduced: both branches return what DuplicateRight returns).  Else matrixMultiplyGeneral (helper :235-263):
+// join on k, then reduce by (i, j) in ascending k.
+std::vector<OutPlan> plan_multiply(const mr_matrix* left, const mr_matrix* right, bool outer, bool mv) {
+  std::vector<OutPlan> plans;
+  std::map<std::pair<int32_t, int32_t>, size_t> index;
+  auto add_pair = [&](int32_t rid, int32_t cid, const Block& a, const Block& b, int32_t k, int32_t kb) {
     // shape checks: BLAS.gemmddd / gemmsdd `require`s (BLAS.scala:338-343, 363-366)
     MR_REQUIRE(a.numCols == b.numRows, MR_EDIM, "The columns of A don't match the rows of B. A: %d, B: %d", a.numCols,
                b.numRows);
+    auto it = index.find({rid, cid});
+    if (it == index.end()) {
+      it = index.emplace(std::make_pair(rid, cid), plans.size()).first;
+      plans.emplace_back();
+    } else if (outer) {
+      plans[it->second] = OutPlan();
+    }
+    OutPlan& o = plans[it->second];
+    o.rid = rid;
+    o.cid = cid;
     if (o.m < 0) {
       o.m = a.numRows;
       o.n = b.numCols;
@@ -91,74 +98,133 @@ struct MultiplyPlanner {
                  "Matrix A and B must have the same number of cols. But found A.numCols = %d, B.numCols = %d", o.n,
                  b.numCols);
     }
-    if (mv) {
-      o.mv.push_back(GemmSrc{&a, &b, k});
-      return;
+    Route r = ROUTE_MV;  // the matrix x vector route keeps every pair as it is
+    if (!mv) {
+      const int kind = pair_kind(a, b);
+      r = kind == PAIR_SPMM ? ROUTE_SPMM : kind == PAIR_SPSP ? ROUTE_SPSP : dspmm_candidate(a, b) ? ROUTE_DSPMM : ROUTE_GEMM;
     }
-    const int kind = pair_kind(a, b);
-    if (kind == PAIR_GEMM && dspmm_candidate(a, b)) {
-      o.cand.push_back(OutPlan::Cand{&a, &b, k, o.gemm.size()});
-    } else if (kind == PAIR_GEMM) {
-      push_gemm(o, dense_of(a), dense_of(b), k);
-    } else if (kind == PAIR_SPMM) {
-      o.spmm.emplace_back(&a, &dense_of(b));  // the n == 1 SpMV case is the same kernel
-    } else {
-      o.spsp.emplace_back(&a, &b);  // LocalMatrix.multiplySparseSparse (:909-911, :143-323): see run_sparse_chains
+    o.pairs.push_back(PlanPair{&a, &b, k, kb, r});
+  };
+  if (outer) {
+    for (auto& l : left->blocks)
+      for (auto& r : right->blocks) add_pair(l.first.first, r.first.second, l.second, r.second, l.first.second, r.first.first);
+  } else {
+    std::map<int32_t, std::vector<std::pair<int32_t, const Block*>>> rights;  // k -> (j, B(k,j))
+    for (auto& r : right->blocks) rights[r.first.first].push_back({r.first.second, &r.second});
+    // left->blocks is ordered by (i, k): iterating it visits k ascending within each i
+    for (auto& l : left->blocks) {
+      auto rit = rights.find(l.first.second);
+      if (rit == rights.end()) continue;
+      for (auto& jb : rit->second) add_pair(l.first.first, jb.first, l.second, *jb.second, l.first.second, l.first.second);
     }
   }
-
-  // Once every pair of o is known: its route candidates take the route when o has no pair on the dense engines, else they are
-  // densified into their places among the GEMM pairs (the summation order of the product without the route).
-  void resolve(OutPlan& o) {
-    if (o.gemm.empty()) {
-      for (const OutPlan::Cand& c : o.cand) o.dspmm.emplace_back(c.a, c.b);
-    } else {
-      size_t shift = 0;
-      for (const OutPlan::Cand& c : o.cand) push_gemm(o, *c.a, dense_of(*c.b), c.k, c.pos + shift++);
-    }
-    o.cand.clear();
+  // Dense x sparse candidates take the stored-entry route only in a block with no pair on the dense engines, else they are
+  // densified in their places among its GEMM pairs (the summation order of the product without the route).  Low-density sparse x
+  // sparse pairs next to any other partial make a dense block sum whatever the partial's own format (LocalMatrix.add), so there
+  // they are sparse x dense products of the densified right operand; a block made of such pairs ONLY replays the reference's
+  // format rules (run_sparse_chains).
+  for (OutPlan& o : plans) {
+    const bool gemm = o.has(ROUTE_GEMM);
+    for (PlanPair& p : o.pairs)
+      if (gemm && p.route == ROUTE_DSPMM) p.route = ROUTE_GEMM;
+    if (!o.only(ROUTE_SPSP))
+      for (PlanPair& p : o.pairs)
+        if (p.route == ROUTE_SPSP) p.route = ROUTE_SPSP_SPMM;
   }
+  return plans;
+}
 
-  void push_gemm(OutPlan& o, const Block& a, const Block& b, int32_t k, size_t pos = SIZE_MAX) {
-    GemmPair p{};
-    p.A = a.values.ptr<double>();
-    p.B = b.values.ptr<double>();
-    p.aT = a.isT;
-    p.bT = b.isT;
-    p.lda = a.isT ? a.numCols : a.numRows;  // BLAS.scala:335
-    p.ldb = b.isT ? b.numCols : b.numRows;  // BLAS.scala:336
-    p.kdim = a.numCols;
-    p.tmA = p.tmB = -1;
-    pos = std::min(pos, o.gemm.size());
-    o.gemm.insert(o.gemm.begin() + static_cast<std::ptrdiff_t>(pos), p);
-    o.src.insert(o.src.begin() + static_cast<std::ptrdiff_t>(pos), GemmSrc{&a, &b, k});
+// What the plans decide for the whole product: the DMMA tile variant (large tiles unless they cannot fill the 132 SMs), and
+// whether to try the Ozaki-II engine (gemm_algo 4, or auto with >= 2^33 flop; a block with sparse partials next to dense ones
+// keeps the whole product off it).
+MultiplyDecisions decide(const mr_context* ctx, const std::vector<OutPlan>& plans, int mv) {
+  MultiplyDecisions d;
+  d.mv = mv;
+  int64_t flops = 0, tiles128 = 0;
+  bool mixed = false;
+  for (const OutPlan& o : plans) {
+    if (!o.has(ROUTE_GEMM) || o.m == 0 || o.n == 0) continue;
+    for (const PlanPair& p : o.pairs)
+      if (p.route == ROUTE_GEMM) flops += 2ll * p.a->numRows * p.b->numCols * p.a->numCols;
+    tiles128 += static_cast<int64_t>((o.m + 127) / 128) * ((o.n + 127) / 128);
+    mixed = mixed || !o.only(ROUTE_GEMM);
+  }
+  d.variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
+  d.oz2 = !mixed && (ctx->gemm_algo == 4 || (ctx->gemm_algo == 0 && flops >= (1ll << 33)));
+  return d;
+}
+
+// The dense images the routes read (GEMM operands, right operands of sparse x dense pairs), made once per sparse block; the pairs
+// then point at them.  `temps` keeps them alive until the launches are enqueued (a deque: growth must not move them).
+void densify_operands(mr_context* ctx, std::vector<OutPlan>& plans, std::deque<Block>& temps) {
+  std::map<const Block*, const Block*> densified;
+  auto dense_of = [&](const Block* b) {
+    if (b->dense()) return b;
+    auto it = densified.find(b);
+    if (it == densified.end()) {
+      temps.push_back(densify(ctx, *b));
+      it = densified.emplace(b, &temps.back()).first;
+    }
+    return it->second;
+  };
+  for (OutPlan& o : plans)
+    for (PlanPair& p : o.pairs)
+      if (p.route == ROUTE_GEMM) {
+        p.a = dense_of(p.a);
+        p.b = dense_of(p.b);
+      } else if (p.route == ROUTE_SPMM || p.route == ROUTE_SPSP_SPMM) {
+        p.b = dense_of(p.b);
+      }
+}
+
+// Times the launches enqueued between its construction and stop() when the time_kernels option is on: last_gemm_ms is that time,
+// gemm_ms_total accumulates it.
+struct KernelTimer {
+  mr_context* ctx;
+  explicit KernelTimer(mr_context* c) : ctx(c) {
+    if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
+  }
+  void stop() {
+    if (!ctx->time_kernels) return;
+    CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
+    CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
+    float ms = 0.f;
+    CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+    ctx->stats.last_gemm_ms = ms;
+    ctx->stats.gemm_ms_total += ms;
   }
 };
 
+// Consecutive slots 0, 1, ... of the block rows and the block columns that hold the output blocks plans[i], i in `outs` (a rank
+// of the process grid owns every pr-th block row and pc-th block column: slicing and multiplying the absent ones would only
+// produce zeros).
+void compact_slots(const std::vector<OutPlan>& plans, const std::vector<size_t>& outs, std::map<int32_t, int>& crow,
+                   std::map<int32_t, int>& ccol) {
+  for (size_t i : outs) {
+    crow.emplace(plans[i].rid, 0);
+    ccol.emplace(plans[i].cid, 0);
+  }
+  int s = 0;
+  for (auto& kv : crow) kv.second = s++;
+  s = 0;
+  for (auto& kv : ccol) kv.second = s++;
+}
+
 // gemm_algo 2: the dense pairs of every output block through the wgmma int8 Ozaki pipeline (gemm_ozaki.cu).
 // Returns false when the problem does not fit its regular-grid assumptions or holds Inf/NaN (caller uses DMMA).
-bool try_ozaki(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<double*>& cptr, int32_t blkSize, int64_t M,
+bool try_ozaki(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, int32_t blkSize, int64_t M,
                int64_t K, int64_t N, bool outer) {
   const bool tf32 = ctx->gemm_algo == 3;
   const int S_eff = std::min(7, std::max(2, ctx->ozaki_slices > 0 ? ctx->ozaki_slices : 7));
   // s32 accumulator bound: up to S pairs x K terms of |digit product| <= 2^14 land in one accumulator
   if (M <= 0 || K <= 0 || N <= 0 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX / 2) return false;
   if (!tf32 && K * S_eff >= (1 << 17)) return false;
-  // Compact the block rows / columns that actually have output blocks (a rank of the process grid owns every pr-th
-  // block row and pc-th block column: slicing and multiplying the absent ones would only produce zeros).
-  std::map<int32_t, int32_t> crow, ccol;
-  for (const OutPlan& o : plans)
-    if (!o.gemm.empty()) {
-      crow.emplace(o.rid, 0);
-      ccol.emplace(o.cid, 0);
-    }
+  std::vector<size_t> outs;
+  for (size_t i = 0; i < plans.size(); ++i)
+    if (plans[i].has(ROUTE_GEMM)) outs.push_back(i);
+  std::map<int32_t, int> crow, ccol;
+  compact_slots(plans, outs, crow, ccol);
   if (crow.empty()) return false;
-  {
-    int32_t i = 0;
-    for (auto& kv : crow) kv.second = i++;
-    i = 0;
-    for (auto& kv : ccol) kv.second = i++;
-  }
   const int64_t nbr = static_cast<int64_t>(crow.size()), nbc = static_cast<int64_t>(ccol.size());
   if (nbr * nbc > (1 << 24)) return false;
   const int64_t last_r = crow.rbegin()->first, last_c = ccol.rbegin()->first;
@@ -168,16 +234,15 @@ bool try_ozaki(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<d
   std::vector<double*> ctab(static_cast<size_t>(nbr * nbc), nullptr);
   std::map<const Block*, int> ia, ib;
   std::vector<OzakiOperand> va, vb;
-  for (size_t i = 0; i < plans.size(); ++i) {
+  for (size_t i : outs) {
     const OutPlan& o = plans[i];
-    if (o.gemm.empty()) continue;
     const int32_t cr = crow[o.rid], cc = ccol[o.cid];
     // every block row / column but the last must be a full blkSize tall / wide (the kernel finds blocks by division)
     if (o.m != ((o.rid == last_r) ? Mc - (nbr - 1) * blkSize : blkSize) || o.n != ((o.cid == last_c) ? Nc - (nbc - 1) * blkSize : blkSize))
       return false;
-    if (!o.spmm.empty()) return false;  // mixed dense / sparse partial sums stay on the exact path
+    if (o.has_spmm()) return false;  // mixed dense / sparse partial sums stay on the exact path
     ctab[static_cast<size_t>(cr) * nbc + cc] = cptr[i];
-    for (const GemmSrc& g : o.src) {
+    for (const PlanPair& g : o.pairs) {
       const int64_t k0 = outer ? 0 : static_cast<int64_t>(g.k) * blkSize;
       if (k0 + g.a->numCols > K || g.a->numCols != g.b->numRows) return false;
       if (!ia.count(g.a)) {
@@ -194,7 +259,7 @@ bool try_ozaki(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<d
   }
   if (va.empty() || vb.empty()) return false;
   int launches = 0, nonfinite = 0;
-  if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
+  KernelTimer timer(ctx);
   if (tf32)
     CUDA_CHECK(tf32x3_gemm(va.data(), static_cast<int>(va.size()), vb.data(), static_cast<int>(vb.size()), Mc, K, Nc, ctab.data(),
                            blkSize, static_cast<int>(nbr), static_cast<int>(nbc), &launches, ctx->stream));
@@ -205,14 +270,7 @@ bool try_ozaki(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<d
   note_launch(ctx, launches);
   if (nonfinite) return false;
   ctx->stats.gemm_launches += 1;
-  if (ctx->time_kernels) {
-    CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
-    CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
-    float ms = 0.f;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-    ctx->stats.last_gemm_ms = ms;
-    ctx->stats.gemm_ms_total += ms;
-  }
+  timer.stop();
   return true;
 }
 
@@ -294,27 +352,20 @@ struct Oz2Run {
     const int T = oz2_moduli_for(K, ctx->crt_moduli);
     const int ss = (blk + kOz2TileM - 1) / kOz2TileM * kOz2TileM;
     std::map<int32_t, int> crow, ccol;
-    for (size_t oi : out_plan) {
-      crow.emplace(plans[oi].rid, 0);
-      ccol.emplace(plans[oi].cid, 0);
-    }
-    int i = 0;
-    for (auto& kv : crow) kv.second = i++;
-    i = 0;
-    for (auto& kv : ccol) kv.second = i++;
+    compact_slots(plans, out_plan, crow, ccol);
     const int nr = static_cast<int>(crow.size()), nc = static_cast<int>(ccol.size());
     if (static_cast<int64_t>(nr) * ss > INT32_MAX / 2 || static_cast<int64_t>(nc) * ss > INT32_MAX / 2) return false;
     std::vector<int32_t> rdim(nr, -1), cdim(nc, -1);
-    std::vector<std::vector<const GemmSrc*>> asrc(nr), bsrc(nc);  // unique blocks per block row / column
+    std::vector<std::vector<const PlanPair*>> asrc(nr), bsrc(nc);  // unique blocks per block row / column
     std::map<const Block*, int> seen_a, seen_b;
     for (size_t oi : out_plan) {
       const OutPlan& o = plans[oi];
-      if (!o.spmm.empty() || !o.spsp.empty() || o.m <= 0 || o.n <= 0 || o.m > blk || o.n > blk) return false;
+      if (!o.only(ROUTE_GEMM) || o.m <= 0 || o.n <= 0 || o.m > blk || o.n > blk) return false;
       const int cr = crow[o.rid], cc = ccol[o.cid];
       if (rdim[cr] < 0) rdim[cr] = o.m;
       if (cdim[cc] < 0) cdim[cc] = o.n;
       if (rdim[cr] != o.m || cdim[cc] != o.n) return false;
-      for (const GemmSrc& g : o.src) {
+      for (const PlanPair& g : o.pairs) {
         const int64_t k0 = outer ? 0 : static_cast<int64_t>(g.k) * blk;
         if (g.a->numCols != g.b->numRows || g.a->numCols > blk || k0 + g.a->numCols > K) return false;
         if (g.a->numRows != o.m || g.b->numCols != o.n) return false;
@@ -354,7 +405,7 @@ struct Oz2Run {
         const int32_t base = static_cast<int32_t>((slot0 + static_cast<int>(s_)) * ss);
         p.dims.push_back(is_a ? rdim[id] : cdim[id]);
         want += static_cast<int64_t>(is_a ? rdim[id] : cdim[id]) * K;
-        for (const GemmSrc* g : (is_a ? asrc[id] : bsrc[id])) {
+        for (const PlanPair* g : (is_a ? asrc[id] : bsrc[id])) {
           const Block* b = is_a ? g->a : g->b;
           const int32_t k0 = outer ? 0 : g->k * blk;
           p.blocks.push_back(OzakiOperand{b->values.ptr<double>(), b->numRows, b->numCols, is_a ? base : k0, is_a ? k0 : base,
@@ -404,8 +455,8 @@ struct Oz2Run {
     };
     auto add_fix = [&](Job& j, const OutPlan& o, double* C, int rslot, int cslot) {
       if (!guard) return;
-      Oz2FixOut fo{C, o.m, o.n, rslot, cslot, static_cast<int32_t>(j.fsrcs.size()), static_cast<int32_t>(o.src.size())};
-      for (const GemmSrc& g : o.src)
+      Oz2FixOut fo{C, o.m, o.n, rslot, cslot, static_cast<int32_t>(j.fsrcs.size()), static_cast<int32_t>(o.pairs.size())};
+      for (const PlanPair& g : o.pairs)
         j.fsrcs.push_back(Oz2FixSrc{g.a->values.ptr<double>(), g.b->values.ptr<double>(), outer ? 0 : g.k * blk, g.a->numCols, g.a->numRows,
                                     g.b->numCols, static_cast<uint8_t>(g.a->isT), static_cast<uint8_t>(g.b->isT), {0}});
       j.fouts.push_back(fo);
@@ -560,77 +611,40 @@ int partial_format(bool aT, bool bT, int64_t m, int64_t n, int64_t nnz) {
   return cells <= 2 * nnz + n ? FMT_DENSE : FMT_CSC;
 }
 
-void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<size_t>& chains_all,
-                       const std::vector<double*>& cptr, mr_matrix* result) {
-  std::vector<size_t> chains;  // empty output blocks keep the (empty) dense block run_multiply gave them
-  for (size_t i : chains_all)
-    if (plans[i].m > 0 && plans[i].n > 0) chains.push_back(i);
+void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, mr_matrix* result) {
+  std::vector<size_t> chains;  // empty output blocks keep the (empty) dense block allocate_outputs gave them
+  for (size_t i = 0; i < plans.size(); ++i)
+    if (plans[i].has(ROUTE_SPSP) && plans[i].m > 0 && plans[i].n > 0) chains.push_back(i);
   if (chains.empty()) return;
   const size_t nc = chains.size();
   // ---- frames: an all-CSR chain runs as C^T = B^T A^T on the CSR arrays; any other chain in CSC, its CSR operands converted once
   std::vector<char> csr_frame(nc, 1);
   for (size_t c = 0; c < nc; ++c)
-    for (auto& pr : plans[chains[c]].spsp) {
-      wait_ready(ctx, *pr.first);
-      wait_ready(ctx, *pr.second);
-      if (!pr.first->isT || !pr.second->isT) csr_frame[c] = 0;
+    for (const PlanPair& pr : plans[chains[c]].pairs) {
+      wait_ready(ctx, *pr.a);
+      wait_ready(ctx, *pr.b);
+      if (!pr.a->isT || !pr.b->isT) csr_frame[c] = 0;
     }
-  struct Conv {
-    size_t ptr, idx, val, cur;  // byte offsets in the conversion buffer
-  };
-  std::map<const Block*, Conv> conv;
+  std::map<const Block*, size_t> conv;  // CSR operand -> offset of its CSC copy in the conversion buffer
   size_t conv_bytes = 0;
-  auto need_conv = [&](const Block* b) {
-    if (!b->isT || conv.count(b)) return;
-    Conv v;
-    v.ptr = conv_bytes;
-    conv_bytes += align_up(static_cast<size_t>(b->numCols + 1) * sizeof(int32_t));
-    v.idx = conv_bytes;
-    conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(int32_t));
-    v.val = conv_bytes;
-    conv_bytes += align_up(static_cast<size_t>(b->valuesLen) * sizeof(double));
-    v.cur = conv_bytes;
-    conv_bytes += align_up(static_cast<size_t>(b->numCols) * sizeof(int32_t));
-    conv.emplace(b, v);
-  };
   for (size_t c = 0; c < nc; ++c)
     if (!csr_frame[c])
-      for (auto& pr : plans[chains[c]].spsp) {
-        need_conv(pr.first);
-        need_conv(pr.second);
-      }
+      for (const PlanPair& pr : plans[chains[c]].pairs)
+        for (const Block* b : {pr.a, pr.b})
+          if (b->isT && !conv.count(b)) {
+            conv.emplace(b, conv_bytes);
+            conv_bytes += CscLayout(b->numCols, b->valuesLen).bytes;
+          }
   Buf cbuf;
   if (!conv.empty()) {
     cbuf = std::make_shared<DevBuf>(ctx, conv_bytes);
-    CUDA_CHECK(cudaMemsetAsync(cbuf->p, 0, conv_bytes, ctx->stream));
-    char* base = static_cast<char*>(cbuf->p);
-    std::vector<SpTransDesc> td;
-    std::vector<ScanDesc> sd;
-    int max_nnz = 0, max_nl = 0, max_no = 0;
+    std::vector<CsrToCsc> cv;
     for (auto& kv : conv) {
       const Block* b = kv.first;
-      const Conv& v = kv.second;
-      SpTransDesc d{};
-      d.ptr = b->colPtrs.ptr<int32_t>();
-      d.idx = b->rowIndices.ptr<int32_t>();
-      d.val = b->values.ptr<double>();
-      d.nl = b->numRows;
-      d.no = b->numCols;
-      d.nnz = static_cast<int32_t>(b->valuesLen);
-      d.optr = reinterpret_cast<int32_t*>(base + v.ptr);
-      d.oidx = reinterpret_cast<int32_t*>(base + v.idx);
-      d.oval = reinterpret_cast<double*>(base + v.val);
-      d.cur = reinterpret_cast<int32_t*>(base + v.cur);
-      td.push_back(d);
-      sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
-      max_nnz = std::max(max_nnz, d.nnz);
-      max_nl = std::max(max_nl, d.nl);
-      max_no = std::max(max_no, d.no);
+      cv.push_back(CsrToCsc{b->colPtrs.ptr<int32_t>(), b->rowIndices.ptr<int32_t>(), b->values.ptr<double>(), b->numRows, b->numCols,
+                            b->valuesLen, static_cast<char*>(cbuf->p) + kv.second});
     }
-    Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
-    CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
-                              max_nnz, max_nl, max_no, ctx->stream));
-    note_launch(ctx, 4);
+    csr_to_csc(ctx, cv);
   }
   // ---- the chains and their pairs in the frame
   std::vector<SpgemmChain> ch(nc);
@@ -646,7 +660,7 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
     h.m = csr_frame[c] ? o.n : o.m;
     h.n = csr_frame[c] ? o.m : o.n;
     h.pair_begin = static_cast<int32_t>(pairs.size());
-    h.levels = static_cast<int32_t>(o.spsp.size());
+    h.levels = static_cast<int32_t>(o.pairs.size());
     h.count_off = count_total;
     count_total += 2 * h.levels;
     col_total += h.n;
@@ -654,21 +668,21 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
     max_levels = std::max(max_levels, h.levels);
     auto csc_of = [&](const Block* b, const int32_t*& p, const int32_t*& i, const double*& v) {
       if (b->isT && !csr_frame[c]) {
-        const Conv& cv = conv.at(b);
-        char* base = static_cast<char*>(cbuf->p);
-        p = reinterpret_cast<const int32_t*>(base + cv.ptr);
-        i = reinterpret_cast<const int32_t*>(base + cv.idx);
-        v = reinterpret_cast<const double*>(base + cv.val);
+        const char* w = static_cast<const char*>(cbuf->p) + conv.at(b);
+        const CscLayout L(b->numCols, b->valuesLen);
+        p = reinterpret_cast<const int32_t*>(w + L.ptr);
+        i = reinterpret_cast<const int32_t*>(w + L.idx);
+        v = reinterpret_cast<const double*>(w + L.val);
       } else {  // CSC, or (CSR frame) the CSC arrays of the block's transpose
         p = b->colPtrs.ptr<int32_t>();
         i = b->rowIndices.ptr<int32_t>();
         v = b->values.ptr<double>();
       }
     };
-    for (auto& pr : o.spsp) {
+    for (const PlanPair& pr : o.pairs) {
       SpgemmPair q{};
-      const Block* lb = csr_frame[c] ? pr.second : pr.first;
-      const Block* rb = csr_frame[c] ? pr.first : pr.second;
+      const Block* lb = csr_frame[c] ? pr.b : pr.a;
+      const Block* rb = csr_frame[c] ? pr.a : pr.b;
       csc_of(lb, q.lp, q.li, q.lv);
       csc_of(rb, q.rp, q.ri, q.rv);
       pairs.push_back(q);
@@ -715,7 +729,7 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
     int64_t s_nnz = 0;
     for (int32_t l = 0; l < ch[c].levels; ++l) {
       s_nnz += cs[l];
-      const int pf = partial_format(o.spsp[l].first->isT, o.spsp[l].second->isT, o.m, o.n, cp[l]);
+      const int pf = partial_format(o.pairs[l].a->isT, o.pairs[l].b->isT, o.m, o.n, cp[l]);
       if (l == 0) fmt[c] = pf;
       else if (fmt[c] == FMT_DENSE || pf == FMT_DENSE) fmt[c] = FMT_DENSE;
       else fmt[c] = static_cast<int64_t>(o.m) * o.n > 2 * s_nnz + o.n + 1 ? FMT_CSC : FMT_DENSE;
@@ -733,18 +747,14 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
       const size_t e = static_cast<size_t>(nnz[c]);
       sparse_total += align_up((static_cast<size_t>(ch[c].n) + 1) * sizeof(int32_t)) + align_up(e * sizeof(int32_t)) +
                       align_up(e * sizeof(double));
-      if (via_csr)
-        sparse_total += 2 * align_up((static_cast<size_t>(o.n) + 1) * sizeof(int32_t)) + align_up(e * sizeof(int32_t)) +
-                        align_up(e * sizeof(double));
+      if (via_csr) sparse_total += CscLayout(o.n, nnz[c]).bytes;
     }
   }
   std::unique_ptr<Slab> dslab, sslab;
   if (dense_total) dslab.reset(new Slab(ctx, dense_total));
   if (sparse_total) sslab.reset(new Slab(ctx, sparse_total));
   std::vector<ScanDesc> scans;
-  std::vector<SpTransDesc> finals;
-  std::vector<ScanDesc> final_scans;
-  int fmax_nnz = 0, fmax_nl = 0, fmax_no = 0;
+  std::vector<CsrToCsc> finals;
   for (size_t c = 0; c < nc; ++c) {
     const OutPlan& o = plans[chains[c]];
     SpgemmChain& h = ch[c];
@@ -774,28 +784,12 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
     b.numCols = o.n;
     b.valuesLen = static_cast<int64_t>(e);
     if (csr_frame[c] && fmt[c] == FMT_CSC) {  // CSR arrays of C -> CSC
-      Span cptr2 = sslab->take((static_cast<size_t>(o.n) + 1) * sizeof(int32_t)), cidx = sslab->take(e * sizeof(int32_t)),
-           cval = sslab->take(e * sizeof(double)), cur = sslab->take(static_cast<size_t>(o.n) * sizeof(int32_t));
-      SpTransDesc d{};
-      d.ptr = ptr.ptr<int32_t>();
-      d.idx = idx.ptr<int32_t>();
-      d.val = val.ptr<double>();
-      d.nl = o.m;
-      d.no = o.n;
-      d.nnz = static_cast<int32_t>(e);
-      d.optr = cptr2.ptr<int32_t>();
-      d.oidx = cidx.ptr<int32_t>();
-      d.oval = cval.ptr<double>();
-      d.cur = cur.ptr<int32_t>();
-      finals.push_back(d);
-      final_scans.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
-      fmax_nnz = std::max(fmax_nnz, d.nnz);
-      fmax_nl = std::max(fmax_nl, d.nl);
-      fmax_no = std::max(fmax_no, d.no);
-      CUDA_CHECK(cudaMemsetAsync(d.cur, 0, static_cast<size_t>(o.n) * sizeof(int32_t), ctx->stream));
-      b.colPtrs = cptr2;
-      b.rowIndices = cidx;
-      b.values = cval;
+      const CscLayout L(o.n, b.valuesLen);
+      const Span w = sslab->take(L.bytes);
+      finals.push_back(CsrToCsc{ptr.ptr<int32_t>(), idx.ptr<int32_t>(), val.ptr<double>(), o.m, o.n, b.valuesLen, w.ptr<char>()});
+      b.colPtrs = Span{w.buf, w.off + L.ptr};
+      b.rowIndices = Span{w.buf, w.off + L.idx};
+      b.values = Span{w.buf, w.off + L.val};
       b.colPtrsLen = o.n + 1;
       b.isT = false;
     } else {  // the frame's arrays are the result's: CSC (CSC frame) or CSR (CSR frame)
@@ -818,12 +812,7 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
                            static_cast<const SpgemmChain*>(d_ch2->p), static_cast<const SpgemmPair*>(d_pairs->p), d_counts, d_products,
                            scratch ? scratch->p : nullptr, max_m, shape, ctx->stream));
   note_launch(ctx);
-  if (!finals.empty()) {
-    Buf d_f = upload(ctx, finals), d_fs = upload(ctx, final_scans);
-    CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_f->p), static_cast<const ScanDesc*>(d_fs->p), static_cast<int>(finals.size()),
-                              fmax_nnz, fmax_nl, fmax_no, ctx->stream));
-    note_launch(ctx, 4);
-  }
+  csr_to_csc(ctx, finals);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -833,13 +822,13 @@ void run_sparse_chains(mr_context* ctx, std::vector<OutPlan>& plans, const std::
 // EW_COPY into the scratch).  A flag pass over the A images and a fix-up after the partials give the NaN of a non-finite A(i, k)
 // meeting an implicit zero of S, as the dense image does.  No host synchronisation.
 // ------------------------------------------------------------------------------------------------
-void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::vector<double*>& cptr) {
+void run_dense_sparse(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr) {
   std::vector<size_t> routed;
   for (size_t i = 0; i < plans.size(); ++i)
-    if (!plans[i].dspmm.empty() && plans[i].m > 0 && plans[i].n > 0) routed.push_back(i);
+    if (plans[i].has(ROUTE_DSPMM) && plans[i].m > 0 && plans[i].n > 0) routed.push_back(i);
   if (routed.empty()) return;
   // ---- scratch: one buffer (CSC copies of CSR blocks, prepared segments, column-major images, non-finite sets), and one small
-  // zero-filled one (sptrans cursors, the per-block "any non-finite" flags)
+  // zero-filled one (the per-block "any non-finite" flags)
   size_t bytes = 0, zbytes = 0;
   auto take = [](size_t& total, size_t n) {
     const size_t off = total;
@@ -847,7 +836,7 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
     return off;
   };
   struct SInfo {
-    size_t ptr = 0, idx = 0, val = 0, cur = 0;  // CSC copy of a CSR block
+    size_t csc = 0;  // CSC copy of a CSR block
     size_t ent = 0, rp = 0, seg = 0, kref = 0;
   };
   struct AInfo {
@@ -858,18 +847,14 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
   std::map<const Block*, AInfo> ainfo;
   std::vector<const Block*> sorder, aorder;
   for (size_t i : routed)
-    for (auto& pr : plans[i].dspmm) {
-      const Block &a = *pr.first, &sb = *pr.second;
+    for (const PlanPair& pr : plans[i].pairs) {
+      if (pr.route != ROUTE_DSPMM) continue;
+      const Block &a = *pr.a, &sb = *pr.b;
       wait_ready(ctx, a);
       wait_ready(ctx, sb);
       if (!sinfo.count(&sb)) {
         SInfo v;
-        if (sb.isT) {
-          v.ptr = take(bytes, static_cast<size_t>(sb.numCols + 1) * sizeof(int32_t));
-          v.idx = take(bytes, static_cast<size_t>(sb.valuesLen) * sizeof(int32_t));
-          v.val = take(bytes, static_cast<size_t>(sb.valuesLen) * sizeof(double));
-          v.cur = take(zbytes, static_cast<size_t>(sb.numCols) * sizeof(int32_t));
-        }
+        if (sb.isT) v.csc = take(bytes, CscLayout(sb.numCols, sb.valuesLen).bytes);
         size_t eo, ro, so, ko;
         const size_t aux = take(bytes, dspmm_aux_bytes(sb.numCols, sb.numRows, sb.valuesLen, &eo, &ro, &so, &ko));
         v.ent = aux + eo;
@@ -896,10 +881,11 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
   char* const zbase = static_cast<char*>(zero->p);
   auto csc_of = [&](const Block* sb, const int32_t*& ptr, const int32_t*& idx, const double*& val) {
     if (sb->isT) {
-      const SInfo& v = sinfo.at(sb);
-      ptr = reinterpret_cast<const int32_t*>(base + v.ptr);
-      idx = reinterpret_cast<const int32_t*>(base + v.idx);
-      val = reinterpret_cast<const double*>(base + v.val);
+      const char* w = base + sinfo.at(sb).csc;
+      const CscLayout L(sb->numCols, sb->valuesLen);
+      ptr = reinterpret_cast<const int32_t*>(w + L.ptr);
+      idx = reinterpret_cast<const int32_t*>(w + L.idx);
+      val = reinterpret_cast<const double*>(w + L.val);
     } else {
       ptr = sb->colPtrs.ptr<int32_t>();
       idx = sb->rowIndices.ptr<int32_t>();
@@ -910,37 +896,14 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
     const AInfo& v = ainfo.at(a);
     return v.copy ? reinterpret_cast<const double*>(base + v.img) : a->values.ptr<double>();
   };
-  // ---- CSR right blocks -> CSC (indices ascending; a repeated coordinate's entries end up next to each other, last stored first)
+  // ---- CSR right blocks -> CSC
   {
-    std::vector<SpTransDesc> td;
-    std::vector<ScanDesc> sd;
-    int max_nnz = 0, max_nl = 0, max_no = 0;
-    for (const Block* sb : sorder) {
-      if (!sb->isT) continue;
-      const SInfo& v = sinfo.at(sb);
-      SpTransDesc d{};
-      d.ptr = sb->colPtrs.ptr<int32_t>();
-      d.idx = sb->rowIndices.ptr<int32_t>();
-      d.val = sb->values.ptr<double>();
-      d.nl = sb->numRows;
-      d.no = sb->numCols;
-      d.nnz = static_cast<int32_t>(sb->valuesLen);
-      d.optr = reinterpret_cast<int32_t*>(base + v.ptr);
-      d.oidx = reinterpret_cast<int32_t*>(base + v.idx);
-      d.oval = reinterpret_cast<double*>(base + v.val);
-      d.cur = reinterpret_cast<int32_t*>(zbase + v.cur);
-      td.push_back(d);
-      sd.push_back(ScanDesc{d.cur, d.optr, d.no, 0});
-      max_nnz = std::max(max_nnz, d.nnz);
-      max_nl = std::max(max_nl, d.nl);
-      max_no = std::max(max_no, d.no);
-    }
-    if (!td.empty()) {
-      Buf d_td = upload(ctx, td), d_sd = upload(ctx, sd);
-      CUDA_CHECK(launch_sptrans(static_cast<const SpTransDesc*>(d_td->p), static_cast<const ScanDesc*>(d_sd->p), static_cast<int>(td.size()),
-                                max_nnz, max_nl, max_no, ctx->stream));
-      note_launch(ctx, 4);
-    }
+    std::vector<CsrToCsc> cv;
+    for (const Block* sb : sorder)
+      if (sb->isT)
+        cv.push_back(CsrToCsc{sb->colPtrs.ptr<int32_t>(), sb->rowIndices.ptr<int32_t>(), sb->values.ptr<double>(), sb->numRows,
+                              sb->numCols, sb->valuesLen, base + sinfo.at(sb).csc});
+    csr_to_csc(ctx, cv);
   }
   // ---- segments of S^T (one prepared copy per right block)
   {
@@ -1017,10 +980,10 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
     fo.m = o.n;
     fo.n = o.m;
     fo.pair_begin = static_cast<int32_t>(pairs.size());
-    fo.pair_count = static_cast<int32_t>(o.dspmm.size());
-    fo.accumulate = o.spmm.empty() ? 0 : 1;  // the block's sparse x dense partials ran before
-    for (auto& pr : o.dspmm) {
-      const Block &a = *pr.first, &sb = *pr.second;
+    fo.accumulate = o.has_spmm() ? 1 : 0;  // the block's sparse x dense partials ran before
+    for (const PlanPair& pr : o.pairs) {
+      if (pr.route != ROUTE_DSPMM) continue;
+      const Block &a = *pr.a, &sb = *pr.b;
       const SInfo& v = sinfo.at(&sb);
       const AInfo& av = ainfo.at(&a);
       DspmmPair dp{};
@@ -1045,6 +1008,7 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
       ctx->stats.dspmm_pairs += 1;
       ctx->stats.dspmm_products += sb.valuesLen * a.numRows;
     }
+    fo.pair_count = static_cast<int32_t>(pairs.size()) - fo.pair_begin;
     const int32_t oi = static_cast<int32_t>(outs.size());
     outs.push_back(fo);
     for (int st = 0; st * kSpmm2StripRows < o.n; ++st)
@@ -1057,18 +1021,11 @@ void run_dense_sparse(mr_context* ctx, std::vector<OutPlan>& plans, const std::v
   std::vector<Spmm2Item> sorted(items.size());
   for (size_t t = 0; t < items.size(); ++t) sorted[t] = items[t].it;
   Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_items = upload(ctx, sorted), d_fix = upload(ctx, fixes);
-  if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
+  KernelTimer timer(ctx);
   CUDA_CHECK(launch_dspmm(static_cast<const Spmm2Item*>(d_items->p), static_cast<int>(sorted.size()), static_cast<const Spmm2Out*>(d_outs->p),
                           static_cast<const DspmmPair*>(d_pairs->p), ctx->stream));
   note_launch(ctx);
-  if (ctx->time_kernels) {
-    CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
-    CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
-    float ms = 0.f;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-    ctx->stats.last_gemm_ms = ms;
-    ctx->stats.gemm_ms_total += ms;
-  }
+  timer.stop();
   CUDA_CHECK(launch_ds_fixup(static_cast<const DsFixPair*>(d_fix->p), static_cast<int>(fixes.size()), ctx->stream));
   note_launch(ctx);
 }
@@ -1112,7 +1069,7 @@ void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::v
   int max_nlines = 0, max_across = 0, max_cols = 1;
   for (size_t i = 0; i < plans.size(); ++i) {
     const OutPlan& o = plans[i];
-    if (o.mv.empty() || o.m <= 0 || o.n <= 0) continue;
+    if (o.m <= 0 || o.n <= 0) continue;
     const int32_t len = xa ? o.n : o.m, cols = xa ? o.m : o.n;
     max_cols = std::max(max_cols, static_cast<int>(cols));
     MvOut mo{};
@@ -1120,8 +1077,8 @@ void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::v
     mo.len = len;
     mo.cols = cols;
     mo.pair_begin = static_cast<int32_t>(pairs.size());
-    mo.pair_count = static_cast<int32_t>(o.mv.size());
-    for (const GemmSrc& g : o.mv) {
+    mo.pair_count = static_cast<int32_t>(o.pairs.size());
+    for (const PlanPair& g : o.pairs) {
       const Block& a = xa ? *g.b : *g.a;  // the matrix block
       const Block& x = xa ? *g.a : *g.b;  // the thin block: kdim x cols (A X) or cols x kdim (X A), in either layout
       wait_ready(ctx, a);
@@ -1200,26 +1157,11 @@ void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::v
   note_launch(ctx);
 }
 
-void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner& planner, int32_t blkSize,
-                  mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows,
-                  const MultiplyDecisions* decisions, int mv_side) {
+// Allocates all output blocks from one slab (packed in plan order, or at their slots when the result is a sharded dataset), or takes
+// them from the caller's windows.  Returns where each plan's block is written.
+std::vector<double*> allocate_outputs(mr_context* ctx, const std::vector<OutPlan>& plans, mr_matrix* result,
+                                      const OutWindowFn* out_windows) {
   const ShardInfo* out_shard = result->shard.get();
-  // Low-density sparse x sparse pairs: next to any dense partial the block sum is dense whatever the partial's own format
-  // (LocalMatrix.add), so there they are ordinary sparse x dense products of the densified right operand; an output block
-  // made of such pairs ONLY replays the reference's format rules (run_sparse_chains).
-  std::vector<size_t> chains;
-  for (size_t i = 0; i < plans.size(); ++i) {
-    OutPlan& o = plans[i];
-    if (o.spsp.empty()) continue;
-    if (o.gemm.empty() && o.spmm.empty() && o.dspmm.empty()) {
-      chains.push_back(i);
-    } else {
-      for (auto& pr : o.spsp) o.spmm.emplace_back(pr.first, &planner.dense_of(*pr.second));
-      o.spsp.clear();
-    }
-  }
-  // allocate all output blocks from one slab (packed in plan order, or at their slots when the result is a sharded dataset), or
-  // take them from the caller's windows
   std::vector<double*> cptr(plans.size());
   if (out_windows) {
     for (size_t i = 0; i < plans.size(); ++i) {
@@ -1243,7 +1185,7 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
     }
   } else {
     // chain outputs (run_sparse_chains) get their arrays once their format is known: a dense window only if they end dense
-    auto chain_out = [&](const OutPlan& o) { return !o.spsp.empty() && o.m > 0 && o.n > 0; };
+    auto chain_out = [&](const OutPlan& o) { return o.has(ROUTE_SPSP) && o.m > 0 && o.n > 0; };
     size_t total = 0;
     for (auto& o : plans)
       if (!chain_out(o)) total += align_up(static_cast<size_t>(o.m) * o.n * sizeof(double));
@@ -1256,260 +1198,261 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       result->blocks[{o.rid, o.cid}] = dense_block(o.m, o.n, s, false);  // product is never transposed (MLMatrix.scala:101)
     }
   }
-  if (mv_side != MV_NONE) {
-    run_matvec(ctx, plans, cptr, mv_side == MV_XA);
-    return;
-  }
+  return cptr;
+}
 
-  // ---- fused GEMM launch over every output block that has dense pairs
+// The GEMM pairs of every output block on the dense engines: Ozaki-I / 3xTF32 (gemm_algo 2 / 3) when they fit, else ONE fused
+// DMMA launch (chunked while operands are still arriving from the host), behind the Ozaki-II engine when `dec` says to try it.
+void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, const MultiplyDecisions& dec,
+                       int32_t blkSize, mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer) {
   std::vector<GemmOut> outs;
   std::vector<GemmPair> pairs;
   std::vector<size_t> out_plan;
   int64_t flops = 0;
   for (size_t i = 0; i < plans.size(); ++i) {
-    auto& o = plans[i];
-    if (o.gemm.empty() || o.m == 0 || o.n == 0) continue;
+    const OutPlan& o = plans[i];
+    if (!o.has(ROUTE_GEMM) || o.m == 0 || o.n == 0) continue;
     GemmOut go{};
     go.C = cptr[i];
     go.m = o.m;
     go.n = o.n;
     go.pair_begin = static_cast<int32_t>(pairs.size());
-    go.pair_count = static_cast<int32_t>(o.gemm.size());
-    for (auto& p : o.gemm) {
+    for (const PlanPair& g : o.pairs) {
+      if (g.route != ROUTE_GEMM) continue;
+      GemmPair p{};
+      p.A = g.a->values.ptr<double>();
+      p.B = g.b->values.ptr<double>();
+      p.aT = g.a->isT;
+      p.bT = g.b->isT;
+      p.lda = g.a->isT ? g.a->numCols : g.a->numRows;  // BLAS.scala:335
+      p.ldb = g.b->isT ? g.b->numCols : g.b->numRows;  // BLAS.scala:336
+      p.kdim = g.a->numCols;
+      p.tmA = p.tmB = -1;
       pairs.push_back(p);
       flops += 2ll * o.m * o.n * p.kdim;
     }
+    go.pair_count = static_cast<int32_t>(pairs.size()) - go.pair_begin;
     outs.push_back(go);
     out_plan.push_back(i);
   }
+  if (outs.empty()) return;
   // which dense operands are still being produced on another stream (ingest copies)?
   bool pending = false;
   for (size_t i = 0; i < plans.size() && !pending; ++i)
-    for (const GemmSrc& g : plans[i].src)
-      if ((g.a->ready && !block_done(*g.a)) || (g.b->ready && !block_done(*g.b))) {
+    for (const PlanPair& g : plans[i].pairs)
+      if (g.route == ROUTE_GEMM && ((g.a->ready && !block_done(*g.a)) || (g.b->ready && !block_done(*g.b)))) {
         pending = true;
         break;
       }
   (void)cudaGetLastError();
-  auto wait_all_sources = [&] {
-    for (auto& o : plans)
-      for (const GemmSrc& g : o.src) {
-        wait_ready(ctx, *g.a);
-        wait_ready(ctx, *g.b);
-      }
-  };
   // gemm_algo: 0 = auto (Ozaki-II on wgmma with the range guard when the product is large and regular, else DMMA), 1 = DMMA,
   // 2 = Ozaki-I, 3 = 3xTF32, 4 = Ozaki-II without the range guard
   const int algo = ctx->gemm_algo;
-  bool ozaki_done = false;
-  if (!outs.empty() && (algo == 2 || algo == 3)) {
-    wait_all_sources();
-    ozaki_done = try_ozaki(ctx, plans, cptr, blkSize, M, K, N, outer);
-    if (ozaki_done) ctx->stats.last_gemm_flops = flops;
+  if (algo == 2 || algo == 3) {
+    for (const OutPlan& o : plans)
+      for (const PlanPair& g : o.pairs)
+        if (g.route == ROUTE_GEMM) {
+          wait_ready(ctx, *g.a);
+          wait_ready(ctx, *g.b);
+        }
+    if (try_ozaki(ctx, plans, cptr, blkSize, M, K, N, outer)) {
+      ctx->stats.last_gemm_flops = flops;
+      return;
+    }
   }
-  if (!outs.empty() && !ozaki_done) {
-    // tile shape: large tiles unless they cannot fill the 132 SMs
-    int64_t tiles128 = 0;
-    for (auto& go : outs) tiles128 += static_cast<int64_t>((go.m + 127) / 128) * ((go.n + 127) / 128);
-    int variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
-    if (decisions) variant = decisions->variant;
-    if (ctx->force_variant >= 0) variant = ctx->force_variant;
-    const int BM = gemm_tile_m(variant), BN = gemm_tile_n(variant);
-    const int tpbm = std::max(1, (blkSize + BM - 1) / BM), tpbn = std::max(1, (blkSize + BN - 1) / BN);
-    struct Keyed {
-      int64_t band, gm, gn;
-      GemmTile t;
-    };
-    std::vector<Keyed> keyed;
-    constexpr int kBand = 12;  // the ~132 resident tiles (12 columns x 11 rows) share A row- and B column-panels in L2; carried over, not re-tuned for H100
+  const int variant = ctx->force_variant >= 0 ? ctx->force_variant : dec.variant;
+  const int BM = gemm_tile_m(variant), BN = gemm_tile_n(variant);
+  const int tpbm = std::max(1, (blkSize + BM - 1) / BM), tpbn = std::max(1, (blkSize + BN - 1) / BN);
+  struct Keyed {
+    int64_t band, gm, gn;
+    GemmTile t;
+  };
+  std::vector<Keyed> keyed;
+  constexpr int kBand = 12;  // the ~132 resident tiles (12 columns x 11 rows) share A row- and B column-panels in L2; carried over, not re-tuned for H100
+  for (size_t oi = 0; oi < outs.size(); ++oi) {
+    const OutPlan& o = plans[out_plan[oi]];
+    const int tm = (outs[oi].m + BM - 1) / BM, tn = (outs[oi].n + BN - 1) / BN;
+    for (int a = 0; a < tm; ++a)
+      for (int b = 0; b < tn; ++b) {
+        const int64_t gm = static_cast<int64_t>(o.rid) * tpbm + a, gn = static_cast<int64_t>(o.cid) * tpbn + b;
+        keyed.push_back({gn / kBand, gm, gn, GemmTile{static_cast<int32_t>(oi), a, b, 0}});
+      }
+  }
+  // Chunked launch when operands are still arriving from the host: one launch per block row of C, each waiting
+  // only for the A row panel it reads (and all of B), so compute overlaps the remaining ingest and the egress of
+  // finished rows.  With resident operands it is ONE launch.
+  // Chunk key of an output block = ingest sequence number of the LAST operand block it needs that is still in flight
+  // (the ingest stream is in order, so waiting for that one copy implies all earlier ones).  Output blocks are
+  // launched in key order, in chunks of >= ~8 waves of tiles, so whatever has landed is multiplied while the rest of
+  // A and B is still on the wire -- row panels, column panels or an interleaving of both, whatever order the caller
+  // uploaded them in.
+  const bool chunked = pending && ctx->pipeline != 0;
+  std::vector<int> group_of(outs.size(), 0);
+  int ngroups_dyn = 1;
+  if (chunked) {
+    std::vector<std::pair<uint64_t, size_t>> order(outs.size());
     for (size_t oi = 0; oi < outs.size(); ++oi) {
-      const OutPlan& o = plans[out_plan[oi]];
-      const int tm = (outs[oi].m + BM - 1) / BM, tn = (outs[oi].n + BN - 1) / BN;
-      for (int a = 0; a < tm; ++a)
-        for (int b = 0; b < tn; ++b) {
-          const int64_t gm = static_cast<int64_t>(o.rid) * tpbm + a, gn = static_cast<int64_t>(o.cid) * tpbn + b;
-          keyed.push_back({gn / kBand, gm, gn, GemmTile{static_cast<int32_t>(oi), a, b, 0}});
+      uint64_t key = 0;
+      for (const PlanPair& g : plans[out_plan[oi]].pairs) {
+        if (g.route != ROUTE_GEMM) continue;
+        if (g.a->ready) key = std::max(key, g.a->seq);
+        if (g.b->ready) key = std::max(key, g.b->seq);
+      }
+      order[oi] = {key, oi};
+    }
+    std::sort(order.begin(), order.end());
+    const int64_t min_tiles = 132;  // >= one wave; the launches overlap on the side streams, so small chunks cost nothing
+    int64_t acc_tiles = 0;
+    int gcur = 0;
+    for (size_t r = 0; r < order.size(); ++r) {
+      const size_t oi = order[r].second;
+      // close the chunk when it is big enough AND the next block waits for a later copy
+      if (acc_tiles >= min_tiles && r > 0 && order[r].first != order[r - 1].first) {
+        ++gcur;
+        acc_tiles = 0;
+      }
+      group_of[oi] = gcur;
+      acc_tiles += static_cast<int64_t>((outs[oi].m + BM - 1) / BM) * ((outs[oi].n + BN - 1) / BN);
+    }
+    ngroups_dyn = gcur + 1;
+  }
+  // The int8 tensor-core path (Ozaki-II residues + CRT) runs group by group in front of the DMMA launches, which then only execute
+  // when the engine's device flag reports operands it cannot represent.  Small products stay on the exact kernel in auto mode.
+  Oz2Run oz2;
+  const bool use_oz2 = dec.oz2 && oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0);
+  auto grp = [&](const Keyed& k) { return group_of[k.t.out]; };
+  std::sort(keyed.begin(), keyed.end(), [&](const Keyed& x, const Keyed& y) {
+    const int gx = grp(x), gy = grp(y);
+    if (gx != gy) return gx < gy;
+    if (x.band != y.band) return x.band < y.band;
+    if (x.gm != y.gm) return x.gm < y.gm;
+    return x.gn < y.gn;
+  });
+  std::vector<GemmTile> tiles(keyed.size());
+  for (size_t i = 0; i < keyed.size(); ++i) tiles[i] = keyed[i].t;
+  // TMA descriptors of the K-contiguous operand blocks (row-major A blocks, column-major B blocks)
+  struct TmapBytes { unsigned char b[128]; };
+  std::vector<TmapBytes> tmaps;
+  std::map<std::tuple<const double*, int64_t, int64_t, int64_t>, int32_t> tmap_index;
+  auto tmap_of = [&](const double* base, int64_t kdim, int64_t rows, int64_t ld, int tile) -> int32_t {
+    auto key = std::make_tuple(base, kdim, rows, ld);
+    auto it = tmap_index.find(key);
+    if (it != tmap_index.end()) return it->second;
+    TmapBytes t;
+    int32_t idx = -1;
+    if (encode_kcontig_tmap(t.b, base, kdim, rows, ld, tile)) {
+      idx = static_cast<int32_t>(tmaps.size());
+      tmaps.push_back(t);
+    }
+    tmap_index.emplace(key, idx);
+    return idx;
+  };
+  for (auto& go : outs)
+    for (int p = go.pair_begin; p < go.pair_begin + go.pair_count; ++p) {
+      GemmPair& pr = pairs[p];
+      if (pr.aT) pr.tmA = tmap_of(pr.A, pr.kdim, go.m, pr.lda, BM);
+      if (!pr.bT) pr.tmB = tmap_of(pr.B, pr.kdim, go.n, pr.ldb, BN);
+    }
+  Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_tiles = upload(ctx, tiles), d_tmaps = upload(ctx, tmaps);
+  if (use_oz2) {
+    oz2.upload_tables();
+    ctx->stats.tc_int8_ops = oz2.int8_ops;
+    ctx->stats.tc_moduli = oz2_moduli(oz2.eng);
+    ctx->stats.tc_gemm_launches += 1;
+  }
+  KernelTimer timer(ctx);
+  const int ngroups = ngroups_dyn;
+  const bool side = chunked && ngroups > 1;
+  if (side) {  // fork: the side streams start after everything enqueued so far (output slab, descriptor tables)
+    CUDA_CHECK(cudaEventRecord(ctx->ev_order, ctx->stream));
+    for (int i = 0; i < mr_context::kChunkStreams; ++i) CUDA_CHECK(cudaStreamWaitEvent(ctx->chunk_stream[i], ctx->ev_order, 0));
+  }
+  size_t t0 = 0;
+  for (int gi = 0; gi < ngroups; ++gi) {
+    size_t t1 = t0;
+    while (t1 < keyed.size() && grp(keyed[t1]) == gi) ++t1;
+    // DMMA chunks are independent launches: round-robin over the side streams so that tails overlap.  The Ozaki-II engine's
+    // jobs share its residue planes and each fills the machine by itself (persistent kernel): one side stream, in order.
+    cudaStream_t cs = side ? ctx->chunk_stream[use_oz2 ? 0 : gi % mr_context::kChunkStreams] : ctx->stream;
+    // wait for exactly the operand blocks this chunk reads
+    std::vector<char> seen(outs.size(), 0);
+    for (size_t t = t0; t < t1; ++t) {
+      const int oi = keyed[t].t.out;
+      if (seen[oi]) continue;
+      seen[oi] = 1;
+      for (const PlanPair& g : plans[out_plan[oi]].pairs) {
+        if (g.route != ROUTE_GEMM) continue;
+        wait_ready_on(cs, *g.a);
+        wait_ready_on(cs, *g.b);
+      }
+    }
+    if (use_oz2) oz2.run_group(gi, cs);
+    CUDA_CHECK(launch_gemm_f64(static_cast<const GemmOut*>(d_outs->p), static_cast<const GemmPair*>(d_pairs->p),
+                               static_cast<const GemmTile*>(d_tiles->p) + t0, static_cast<int>(t1 - t0), d_tmaps->p, variant,
+                               cs, use_oz2 ? oz2.flag() : nullptr));
+    note_launch(ctx);
+    if (chunked) {  // consumers on the egress stream wait for this chunk only
+      ReadyPtr r = std::make_shared<Ready>();
+      CUDA_CHECK(cudaEventRecord(r->ev, cs));
+      for (size_t oi = 0; oi < outs.size(); ++oi)
+        if (seen[oi]) {
+          const OutPlan& o = plans[out_plan[oi]];
+          if (!o.has_spmm()) result->blocks[{o.rid, o.cid}].ready = r;  // blocks with sparse partials finish later
         }
     }
-    // Chunked launch when operands are still arriving from the host: one launch per block row of C, each waiting
-    // only for the A row panel it reads (and all of B), so compute overlaps the remaining ingest and the egress of
-    // finished rows.  With resident operands it is ONE launch.
-    // Chunk key of an output block = ingest sequence number of the LAST operand block it needs that is still in flight
-    // (the ingest stream is in order, so waiting for that one copy implies all earlier ones).  Output blocks are
-    // launched in key order, in chunks of >= ~8 waves of tiles, so whatever has landed is multiplied while the rest of
-    // A and B is still on the wire -- row panels, column panels or an interleaving of both, whatever order the caller
-    // uploaded them in.
-    const bool chunked = pending && ctx->pipeline != 0;
-    std::vector<int> group_of(outs.size(), 0);
-    int ngroups_dyn = 1;
-    if (chunked) {
-      std::vector<std::pair<uint64_t, size_t>> order(outs.size());
-      for (size_t oi = 0; oi < outs.size(); ++oi) {
-        uint64_t key = 0;
-        for (const GemmSrc& g : plans[out_plan[oi]].src) {
-          if (g.a->ready) key = std::max(key, g.a->seq);
-          if (g.b->ready) key = std::max(key, g.b->seq);
-        }
-        order[oi] = {key, oi};
-      }
-      std::sort(order.begin(), order.end());
-      const int64_t min_tiles = 132;  // >= one wave; the launches overlap on the side streams, so small chunks cost nothing
-      int64_t acc_tiles = 0;
-      int gcur = 0;
-      for (size_t r = 0; r < order.size(); ++r) {
-        const size_t oi = order[r].second;
-        // close the chunk when it is big enough AND the next block waits for a later copy
-        if (acc_tiles >= min_tiles && r > 0 && order[r].first != order[r - 1].first) {
-          ++gcur;
-          acc_tiles = 0;
-        }
-        group_of[oi] = gcur;
-        acc_tiles += static_cast<int64_t>((outs[oi].m + BM - 1) / BM) * ((outs[oi].n + BN - 1) / BN);
-      }
-      ngroups_dyn = gcur + 1;
-    }
-    // The int8 tensor-core path (Ozaki-II residues + CRT) runs group by group in front of the DMMA launches, which then only execute
-    // when the engine's device flag reports operands it cannot represent.  Small products stay on the exact kernel in auto mode.
-    Oz2Run oz2;
-    bool use_oz2 = false;
-    if (decisions ? decisions->oz2 : (algo == 4 || (algo == 0 && flops >= (1ll << 33))))
-      use_oz2 = oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0);
-    auto grp = [&](const Keyed& k) { return group_of[k.t.out]; };
-    std::sort(keyed.begin(), keyed.end(), [&](const Keyed& x, const Keyed& y) {
-      const int gx = grp(x), gy = grp(y);
-      if (gx != gy) return gx < gy;
-      if (x.band != y.band) return x.band < y.band;
-      if (x.gm != y.gm) return x.gm < y.gm;
-      return x.gn < y.gn;
-    });
-    std::vector<GemmTile> tiles(keyed.size());
-    for (size_t i = 0; i < keyed.size(); ++i) tiles[i] = keyed[i].t;
-    // TMA descriptors of the K-contiguous operand blocks (row-major A blocks, column-major B blocks)
-    struct TmapBytes { unsigned char b[128]; };
-    std::vector<TmapBytes> tmaps;
-    std::map<std::tuple<const double*, int64_t, int64_t, int64_t>, int32_t> tmap_index;
-    auto tmap_of = [&](const double* base, int64_t kdim, int64_t rows, int64_t ld, int tile) -> int32_t {
-      auto key = std::make_tuple(base, kdim, rows, ld);
-      auto it = tmap_index.find(key);
-      if (it != tmap_index.end()) return it->second;
-      TmapBytes t;
-      int32_t idx = -1;
-      if (encode_kcontig_tmap(t.b, base, kdim, rows, ld, tile)) {
-        idx = static_cast<int32_t>(tmaps.size());
-        tmaps.push_back(t);
-      }
-      tmap_index.emplace(key, idx);
-      return idx;
-    };
-    for (auto& go : outs)
-      for (int p = go.pair_begin; p < go.pair_begin + go.pair_count; ++p) {
-        GemmPair& pr = pairs[p];
-        if (pr.aT) pr.tmA = tmap_of(pr.A, pr.kdim, go.m, pr.lda, BM);
-        if (!pr.bT) pr.tmB = tmap_of(pr.B, pr.kdim, go.n, pr.ldb, BN);
-      }
-    Buf d_outs = upload(ctx, outs), d_pairs = upload(ctx, pairs), d_tiles = upload(ctx, tiles), d_tmaps = upload(ctx, tmaps);
-    if (use_oz2) {
-      oz2.upload_tables();
-      ctx->stats.tc_int8_ops = oz2.int8_ops;
-      ctx->stats.tc_moduli = oz2_moduli(oz2.eng);
-      ctx->stats.tc_gemm_launches += 1;
-    }
-    if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
-    const int ngroups = ngroups_dyn;
-    const bool side = chunked && ngroups > 1;
-    if (side) {  // fork: the side streams start after everything enqueued so far (output slab, descriptor tables)
-      CUDA_CHECK(cudaEventRecord(ctx->ev_order, ctx->stream));
-      for (int i = 0; i < mr_context::kChunkStreams; ++i) CUDA_CHECK(cudaStreamWaitEvent(ctx->chunk_stream[i], ctx->ev_order, 0));
-    }
-    size_t t0 = 0;
-    for (int gi = 0; gi < ngroups; ++gi) {
-      size_t t1 = t0;
-      while (t1 < keyed.size() && grp(keyed[t1]) == gi) ++t1;
-      // DMMA chunks are independent launches: round-robin over the side streams so that tails overlap.  The Ozaki-II engine's
-      // jobs share its residue planes and each fills the machine by itself (persistent kernel): one side stream, in order.
-      cudaStream_t cs = side ? ctx->chunk_stream[use_oz2 ? 0 : gi % mr_context::kChunkStreams] : ctx->stream;
-      // wait for exactly the operand blocks this chunk reads
-      std::vector<char> seen(outs.size(), 0);
-      for (size_t t = t0; t < t1; ++t) {
-        const int oi = keyed[t].t.out;
-        if (seen[oi]) continue;
-        seen[oi] = 1;
-        for (const GemmSrc& g : plans[out_plan[oi]].src) {
-          wait_ready_on(cs, *g.a);
-          wait_ready_on(cs, *g.b);
-        }
-      }
-      if (use_oz2) oz2.run_group(gi, cs);
-      CUDA_CHECK(launch_gemm_f64(static_cast<const GemmOut*>(d_outs->p), static_cast<const GemmPair*>(d_pairs->p),
-                                 static_cast<const GemmTile*>(d_tiles->p) + t0, static_cast<int>(t1 - t0), d_tmaps->p, variant,
-                                 cs, use_oz2 ? oz2.flag() : nullptr));
-      note_launch(ctx);
-      if (chunked) {  // consumers on the egress stream wait for this chunk only
-        ReadyPtr r = std::make_shared<Ready>();
-        CUDA_CHECK(cudaEventRecord(r->ev, cs));
-        for (size_t oi = 0; oi < outs.size(); ++oi)
-          if (seen[oi]) {
-            const OutPlan& o = plans[out_plan[oi]];
-            if (o.spmm.empty()) result->blocks[{o.rid, o.cid}].ready = r;  // blocks with sparse partials finish later
-          }
-      }
-      t0 = t1;
-    }
-    if (side) {  // join: later work on the context stream (and the release of the descriptor tables) follows every chunk
-      for (int i = 0; i < mr_context::kChunkStreams; ++i) {
-        CUDA_CHECK(cudaEventRecord(ctx->chunk_join[i], ctx->chunk_stream[i]));
-        CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->chunk_join[i], 0));
-      }
-    }
-    ctx->stats.gemm_launches += 1;
-    ctx->stats.last_gemm_flops = flops;
-    if (ctx->time_kernels) {
-      CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
-      CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
-      float ms = 0.f;
-      CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-      ctx->stats.last_gemm_ms = ms;
-      ctx->stats.gemm_ms_total += ms;
+    t0 = t1;
+  }
+  if (side) {  // join: later work on the context stream (and the release of the descriptor tables) follows every chunk
+    for (int i = 0; i < mr_context::kChunkStreams; ++i) {
+      CUDA_CHECK(cudaEventRecord(ctx->chunk_join[i], ctx->chunk_stream[i]));
+      CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->chunk_join[i], 0));
     }
   }
+  ctx->stats.gemm_launches += 1;
+  ctx->stats.last_gemm_flops = flops;
+  timer.stop();
+}
 
-  // ---- sparse x dense partial products accumulate onto the GEMM result (LocalMatrix.add of partials).
-  // CSR pairs with block dims <= 1024 go through ONE fused launch (K loop over the pairs inside the kernel): the pipelined
-  // TMA kernel of spmm.cu when the output block is large enough to fill its 512 x 32 tiles and B can be addressed by a tensor
-  // map, else the simple shared-memory kernel of ew.cu; CSC pairs and oversized blocks use the per-pair kernels.
+// ------------------------------------------------------------------------------------------------
+// Sparse x dense partial products, accumulated onto the GEMM result (LocalMatrix.add of partials).  CSR pairs with block dims
+// <= 1024 go through ONE fused launch (K loop over the pairs inside the kernel): the pipelined TMA kernel of spmm.cu when the
+// output block is large enough to fill its 512 x 32 tiles and B can be addressed by a tensor map, else the simple shared-memory
+// kernel of ew.cu; CSC pairs and oversized blocks use the per-pair kernels.  In a block, its own sparse x dense pairs come first
+// in ascending k, then its low-density sparse x sparse ones (the summation order of the densifying reference).
+// ------------------------------------------------------------------------------------------------
+void run_sparse_dense(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr) {
   std::vector<SpmmOut> fouts;
   std::vector<SpmmPair> fpairs;
   int fused_max_n = 0;
   std::vector<Spmm2Out> outs2;
-  std::vector<Spmm2Pair> pairs2;
-  std::vector<Spmm2Prep> preps2;
+  std::vector<std::pair<const Block*, const Block*>> pairs2;  // (S, B) of each pair of the pipelined kernel
   std::vector<Spmm2Item> items2;
   struct Key2 {
     int32_t cid, ctile, rid, strip;
   };
   std::vector<Key2> keys2;
-  std::map<const Block*, int> prep_of;                     // sparse block -> index into preps2
-  std::map<const Block*, int32_t> tmap_of_b;               // dense block -> tensor map index
-  struct TmapBytes2 { unsigned char b[128]; };
-  std::vector<TmapBytes2> tmaps2;
-  std::vector<EwDesc> transposes;                          // column-major B blocks -> row-major scratch
-  std::vector<std::pair<const Block*, size_t>> trans_of;   // (block, offset in the scratch buffer)
-  std::vector<size_t> aux_off;                             // per prep: offset of its aux region
+  // scratch offsets: re-packed CSR segments of every sparse block, row-major copies of the column-major dense blocks
+  struct SegOff {
+    size_t ent, rp, seg;
+  };
+  std::map<const Block*, SegOff> seg_of;
+  std::vector<const Block*> sorder, torder;
+  std::map<const Block*, size_t> trans_of;  // column-major dense block -> offset of its row-major copy
+  std::map<const Block*, int32_t> tmap_of_b;  // dense block -> tensor map index
   size_t aux_total = 0, trans_total = 0;
-  int prep_max_m = 0, prep_max_k = 0, trans_max_r = 0, trans_max_c = 0;
   for (size_t i = 0; i < plans.size(); ++i) {
-    auto& o = plans[i];
-    bool have = !o.gemm.empty();
-    if (o.m == 0 || o.n == 0 || !o.spsp.empty()) continue;
+    const OutPlan& o = plans[i];
+    bool have = o.has(ROUTE_GEMM);
+    if (o.m == 0 || o.n == 0 || o.has(ROUTE_SPSP)) continue;
     std::vector<std::pair<const Block*, const Block*>> slow, fused;
-    for (auto& sp : o.spmm) {
-      const Block& s = *sp.first;
-      const Block& b = *sp.second;
-      wait_ready(ctx, s);
-      wait_ready(ctx, b);
-      if (s.isT && o.m <= kSpmmMaxDim && s.numCols <= kSpmmMaxDim) fused.push_back(sp);
-      else slow.push_back(sp);
-    }
+    for (Route r : {ROUTE_SPMM, ROUTE_SPSP_SPMM})
+      for (const PlanPair& p : o.pairs) {
+        if (p.route != r) continue;
+        wait_ready(ctx, *p.a);
+        wait_ready(ctx, *p.b);
+        if (p.a->isT && o.m <= kSpmmMaxDim && p.a->numCols <= kSpmmMaxDim) fused.emplace_back(p.a, p.b);
+        else slow.emplace_back(p.a, p.b);
+      }
     for (auto& sp : slow) {  // per-pair kernels first so the fused launch can simply accumulate on top
       const Block& s = *sp.first;
       const Block& b = *sp.second;
@@ -1533,48 +1476,22 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       for (auto& sp : fused) {
         const Block& sblk = *sp.first;
         const Block& bblk = *sp.second;
-        auto pit = prep_of.find(&sblk);
-        if (pit == prep_of.end()) {
+        if (!seg_of.count(&sblk)) {
           size_t eo, ro, so;
           const size_t bytes = spmm2_aux_bytes(sblk.numRows, sblk.numCols, sblk.valuesLen, &eo, &ro, &so);
-          Spmm2Prep pp{};
-          pp.ptrs = sblk.colPtrs.ptr<int32_t>();
-          pp.idx = sblk.rowIndices.ptr<int32_t>();
-          pp.vals = sblk.values.ptr<double>();
-          pp.m = sblk.numRows;
-          pp.kdim = sblk.numCols;
-          // offsets for now; rebased on the aux allocation below
-          pp.ent = reinterpret_cast<unsigned char*>(aux_total + eo);
-          pp.rp = reinterpret_cast<int32_t*>(aux_total + ro);
-          pp.segoff = reinterpret_cast<int32_t*>(aux_total + so);
-          aux_off.push_back(aux_total);
+          seg_of.emplace(&sblk, SegOff{aux_total + eo, aux_total + ro, aux_total + so});
           aux_total += bytes;
-          prep_max_m = std::max(prep_max_m, pp.m);
-          prep_max_k = std::max(prep_max_k, pp.kdim);
-          pit = prep_of.emplace(&sblk, static_cast<int>(preps2.size())).first;
-          preps2.push_back(pp);
+          sorder.push_back(&sblk);
         }
         if (!tmap_of_b.count(&bblk)) {
           if (!bblk.isT) {  // column-major: row-major copy in the scratch buffer (one transposing pass per multiply)
-            EwDesc d{};
-            d.A = bblk.values.ptr<double>();
-            d.C = reinterpret_cast<double*>(trans_total);  // offset for now
-            d.rows = bblk.numCols;  // the k x n block read as its n x k transpose, stored row-major (aT): see run_sparse_chains
-            d.cols = bblk.numRows;
-            d.aT = 1;
-            trans_of.emplace_back(&bblk, trans_total);
+            trans_of.emplace(&bblk, trans_total);
             trans_total += align_up(static_cast<size_t>(bblk.numRows) * bblk.numCols * sizeof(double));
-            trans_max_r = std::max(trans_max_r, d.rows);
-            trans_max_c = std::max(trans_max_c, d.cols);
-            transposes.push_back(d);
+            torder.push_back(&bblk);
           }
           tmap_of_b.emplace(&bblk, static_cast<int32_t>(tmap_of_b.size()));
         }
-        Spmm2Pair pr{};
-        pr.ent = reinterpret_cast<const unsigned char*>(static_cast<uintptr_t>(pit->second));  // prep index for now
-        pr.kdim = sblk.numCols;
-        pr.tmB = tmap_of_b[&bblk];
-        pairs2.push_back(pr);
+        pairs2.push_back(sp);
       }
       const int32_t oi = static_cast<int32_t>(outs2.size());
       outs2.push_back(fo);
@@ -1606,92 +1523,112 @@ void run_multiply(mr_context* ctx, std::vector<OutPlan>& plans, MultiplyPlanner&
       fused_max_n = std::max(fused_max_n, o.n);
       have = true;
     }
-    if (!have && o.dspmm.empty()) CUDA_CHECK(cudaMemsetAsync(cptr[i], 0, static_cast<size_t>(o.m) * o.n * sizeof(double), ctx->stream));
+    if (!have && !o.has(ROUTE_DSPMM)) CUDA_CHECK(cudaMemsetAsync(cptr[i], 0, static_cast<size_t>(o.m) * o.n * sizeof(double), ctx->stream));
   }
   if (!fouts.empty()) {
     Buf d_fo = upload(ctx, fouts), d_fp = upload(ctx, fpairs);
-    if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
+    KernelTimer timer(ctx);
     CUDA_CHECK(launch_spmm_fused(static_cast<const SpmmOut*>(d_fo->p), static_cast<int>(fouts.size()),
                                  static_cast<const SpmmPair*>(d_fp->p), fused_max_n, ctx->stream));
     note_launch(ctx);
-    if (ctx->time_kernels) {
-      CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
-      CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
-      float ms = 0.f;
-      CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-      ctx->stats.last_gemm_ms = ms;
-      ctx->stats.gemm_ms_total += ms;
-    }
+    timer.stop();
   }
-  if (!outs2.empty()) {
-    // scratch: re-packed CSR segments of every sparse block, row-major copies of the column-major dense blocks
-    Buf aux = std::make_shared<DevBuf>(ctx, std::max<size_t>(aux_total, 16));
-    Buf trans = std::make_shared<DevBuf>(ctx, std::max<size_t>(trans_total, 16));
-    char* aux_base = static_cast<char*>(aux->p);
-    for (Spmm2Prep& pp : preps2) {
-      pp.ent = reinterpret_cast<unsigned char*>(aux_base + reinterpret_cast<uintptr_t>(pp.ent));
-      pp.rp = reinterpret_cast<int32_t*>(aux_base + reinterpret_cast<uintptr_t>(pp.rp));
-      pp.segoff = reinterpret_cast<int32_t*>(aux_base + reinterpret_cast<uintptr_t>(pp.segoff));
-    }
-    for (Spmm2Pair& pr : pairs2) {
-      const Spmm2Prep& pp = preps2[static_cast<size_t>(reinterpret_cast<uintptr_t>(pr.ent))];
-      pr.ent = pp.ent;
-      pr.rp = pp.rp;
-      pr.segoff = pp.segoff;
-    }
-    std::map<const Block*, const double*> rowmajor;  // dense block -> its row-major image
-    for (size_t t = 0; t < transposes.size(); ++t) {
-      transposes[t].C = reinterpret_cast<double*>(static_cast<char*>(trans->p) + reinterpret_cast<uintptr_t>(transposes[t].C));
-      rowmajor[trans_of[t].first] = transposes[t].C;
-    }
-    tmaps2.resize(tmap_of_b.size());
-    bool maps_ok = true;
-    for (auto& kv : tmap_of_b) {
-      const Block* bb = kv.first;
-      const double* base = bb->isT ? bb->values.ptr<double>() : rowmajor[bb];
-      maps_ok = maps_ok && spmm2_encode_b_tmap(tmaps2[kv.second].b, base, bb->numRows, bb->numCols, bb->numCols);
-    }
-    if (!maps_ok) fail(MR_ECUDA, "cuTensorMapEncodeTiled failed for a dense operand of the sparse x dense multiply");
-    // concurrently resident CTAs share the B panel of one 32-column tile: order by (block column, tile, block row, strip)
-    std::vector<size_t> ord(items2.size());
-    for (size_t t = 0; t < ord.size(); ++t) ord[t] = t;
-    std::sort(ord.begin(), ord.end(), [&](size_t x, size_t y) {
-      const Key2 &a = keys2[x], &b2 = keys2[y];
-      if (a.cid != b2.cid) return a.cid < b2.cid;
-      if (a.ctile != b2.ctile) return a.ctile < b2.ctile;
-      if (a.rid != b2.rid) return a.rid < b2.rid;
-      return a.strip < b2.strip;
-    });
-    std::vector<Spmm2Item> sorted_items(items2.size());
-    for (size_t t = 0; t < ord.size(); ++t) sorted_items[t] = items2[ord[t]];
-    Buf d_preps = upload(ctx, preps2), d_outs2 = upload(ctx, outs2), d_pairs2 = upload(ctx, pairs2), d_items = upload(ctx, sorted_items),
-        d_tmaps2 = upload(ctx, tmaps2);
-    CUDA_CHECK(launch_spmm2_prep(static_cast<const Spmm2Prep*>(d_preps->p), static_cast<int>(preps2.size()), prep_max_m, prep_max_k, ctx->stream));
-    note_launch(ctx);
-    if (!transposes.empty()) {
-      Buf d_tr = upload(ctx, transposes);
-      CUDA_CHECK(launch_ew_batched(EW_COPY, static_cast<const EwDesc*>(d_tr->p), static_cast<int>(transposes.size()), trans_max_r,
-                                   trans_max_c, true, ctx->stream));
-      note_launch(ctx);
-    }
-    if (ctx->time_kernels) CUDA_CHECK(cudaEventRecord(ctx->ev0, ctx->stream));
-    CUDA_CHECK(launch_spmm2(static_cast<const Spmm2Item*>(d_items->p), static_cast<int>(sorted_items.size()),
-                            static_cast<const Spmm2Out*>(d_outs2->p), static_cast<const Spmm2Pair*>(d_pairs2->p), d_tmaps2->p, ctx->stream));
-    note_launch(ctx);
-    if (ctx->time_kernels) {
-      CUDA_CHECK(cudaEventRecord(ctx->ev1, ctx->stream));
-      CUDA_CHECK(cudaEventSynchronize(ctx->ev1));
-      float ms = 0.f;
-      CUDA_CHECK(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-      ctx->stats.last_gemm_ms = ms;
-      ctx->stats.gemm_ms_total += ms;
-    }
-    ctx->stats.gemm_launches += 1;
+  if (outs2.empty()) return;
+  Buf aux = std::make_shared<DevBuf>(ctx, std::max<size_t>(aux_total, 16));
+  Buf trans = std::make_shared<DevBuf>(ctx, std::max<size_t>(trans_total, 16));
+  char* const aux_base = static_cast<char*>(aux->p);
+  char* const trans_base = static_cast<char*>(trans->p);
+  std::vector<Spmm2Prep> preps;
+  int prep_max_m = 0, prep_max_k = 0;
+  for (const Block* s : sorder) {
+    const SegOff& so = seg_of.at(s);
+    Spmm2Prep pp{};
+    pp.ptrs = s->colPtrs.ptr<int32_t>();
+    pp.idx = s->rowIndices.ptr<int32_t>();
+    pp.vals = s->values.ptr<double>();
+    pp.m = s->numRows;
+    pp.kdim = s->numCols;
+    pp.ent = reinterpret_cast<unsigned char*>(aux_base + so.ent);
+    pp.rp = reinterpret_cast<int32_t*>(aux_base + so.rp);
+    pp.segoff = reinterpret_cast<int32_t*>(aux_base + so.seg);
+    prep_max_m = std::max(prep_max_m, pp.m);
+    prep_max_k = std::max(prep_max_k, pp.kdim);
+    preps.push_back(pp);
   }
-  run_dense_sparse(ctx, plans, cptr);
-  run_sparse_chains(ctx, plans, chains, cptr, result);
+  std::vector<Spmm2Pair> spairs;
+  for (auto& sp : pairs2) {
+    const SegOff& so = seg_of.at(sp.first);
+    Spmm2Pair pr{};
+    pr.ent = reinterpret_cast<const unsigned char*>(aux_base + so.ent);
+    pr.rp = reinterpret_cast<const int32_t*>(aux_base + so.rp);
+    pr.segoff = reinterpret_cast<const int32_t*>(aux_base + so.seg);
+    pr.kdim = sp.first->numCols;
+    pr.tmB = tmap_of_b.at(sp.second);
+    spairs.push_back(pr);
+  }
+  std::vector<EwDesc> transposes;
+  int trans_max_r = 0, trans_max_c = 0;
+  for (const Block* b : torder) {
+    EwDesc d{};
+    d.A = b->values.ptr<double>();
+    d.C = reinterpret_cast<double*>(trans_base + trans_of.at(b));
+    d.rows = b->numCols;  // the k x n block read as its n x k transpose, stored row-major (aT): see run_sparse_chains
+    d.cols = b->numRows;
+    d.aT = 1;
+    trans_max_r = std::max(trans_max_r, d.rows);
+    trans_max_c = std::max(trans_max_c, d.cols);
+    transposes.push_back(d);
+  }
+  struct TmapBytes {
+    unsigned char b[128];
+  };
+  std::vector<TmapBytes> tmaps(tmap_of_b.size());
+  bool maps_ok = true;
+  for (auto& kv : tmap_of_b) {
+    const Block* bb = kv.first;
+    const double* base = bb->isT ? bb->values.ptr<double>() : reinterpret_cast<const double*>(trans_base + trans_of.at(bb));
+    maps_ok = maps_ok && spmm2_encode_b_tmap(tmaps[kv.second].b, base, bb->numRows, bb->numCols, bb->numCols);
+  }
+  if (!maps_ok) fail(MR_ECUDA, "cuTensorMapEncodeTiled failed for a dense operand of the sparse x dense multiply");
+  // concurrently resident CTAs share the B panel of one 32-column tile: order by (block column, tile, block row, strip)
+  std::vector<size_t> ord(items2.size());
+  for (size_t t = 0; t < ord.size(); ++t) ord[t] = t;
+  std::sort(ord.begin(), ord.end(), [&](size_t x, size_t y) {
+    const Key2 &a = keys2[x], &b2 = keys2[y];
+    return std::tie(a.cid, a.ctile, a.rid, a.strip) < std::tie(b2.cid, b2.ctile, b2.rid, b2.strip);
+  });
+  std::vector<Spmm2Item> sorted_items(items2.size());
+  for (size_t t = 0; t < ord.size(); ++t) sorted_items[t] = items2[ord[t]];
+  Buf d_preps = upload(ctx, preps), d_outs2 = upload(ctx, outs2), d_pairs2 = upload(ctx, spairs), d_items = upload(ctx, sorted_items),
+      d_tmaps = upload(ctx, tmaps);
+  CUDA_CHECK(launch_spmm2_prep(static_cast<const Spmm2Prep*>(d_preps->p), static_cast<int>(preps.size()), prep_max_m, prep_max_k, ctx->stream));
+  note_launch(ctx);
+  if (!transposes.empty()) {
+    Buf d_tr = upload(ctx, transposes);
+    CUDA_CHECK(launch_ew_batched(EW_COPY, static_cast<const EwDesc*>(d_tr->p), static_cast<int>(transposes.size()), trans_max_r,
+                                 trans_max_c, true, ctx->stream));
+    note_launch(ctx);
+  }
+  KernelTimer timer(ctx);
+  CUDA_CHECK(launch_spmm2(static_cast<const Spmm2Item*>(d_items->p), static_cast<int>(sorted_items.size()),
+                          static_cast<const Spmm2Out*>(d_outs2->p), static_cast<const Spmm2Pair*>(d_pairs2->p), d_tmaps->p, ctx->stream));
+  note_launch(ctx);
+  timer.stop();
+  ctx->stats.gemm_launches += 1;
 }
 
+void run_multiply(mr_context* ctx, const std::vector<OutPlan>& plans, const MultiplyDecisions& dec, int32_t blkSize, mr_matrix* result,
+                  int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows) {
+  const std::vector<double*> cptr = allocate_outputs(ctx, plans, result, out_windows);
+  if (dec.mv != MV_NONE) {
+    run_matvec(ctx, plans, cptr, dec.mv == MV_XA);
+    return;
+  }
+  run_dense_engines(ctx, plans, cptr, dec, blkSize, result, M, K, N, outer);
+  run_sparse_dense(ctx, plans, cptr);
+  run_dense_sparse(ctx, plans, cptr);
+  run_sparse_chains(ctx, plans, cptr, result);
+}
 
 }  // namespace
 
@@ -1704,137 +1641,54 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
   for (auto& kv : right->blocks)
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
-  MultiplyPlanner planner{ctx};
-  const int mv_side = decisions ? decisions->mv
-                                : matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
-  planner.mv = mv_side != MV_NONE;
-  std::vector<OutPlan> plans;
-  const int64_t leftColBlkNum = ceil_div(leftColNum, blkSize);    // MatfastExecution.scala:712
-  const int64_t rightRowBlkNum = ceil_div(rightRowNum, blkSize);  // :713
-  if (leftColBlkNum == 1 && rightRowBlkNum == 1) {
-    // outer-product paths (:714-721 -> helper :175-221): every left block x every right block, no
-    // reduce.  Reference defect B1 (DuplicateLeft throws) is not reproduced; both branches return
-    // what DuplicateRight returns.
-    std::map<std::pair<int32_t, int32_t>, size_t> seen;
-    for (auto& l : left->blocks)
-      for (auto& r : right->blocks) {
-        OutPlan o;
-        o.rid = l.first.first;
-        o.cid = r.first.second;
-        planner.add_pair(o, l.second, r.second, 0);
-        auto key = std::make_pair(o.rid, o.cid);
-        auto it = seen.find(key);
-        if (it == seen.end()) {
-          seen[key] = plans.size();
-          plans.push_back(std::move(o));
-        } else {
-          plans[it->second] = std::move(o);  // duplicate keys: the last row wins when collected into a map
-        }
-      }
-  } else {
-    // matrixMultiplyGeneral (helper :235-263): join on k, then reduce by (i, j) in ascending k.
-    std::map<int32_t, std::vector<std::pair<int32_t, const Block*>>> rights;  // k -> (j, B(k,j))
-    for (auto& r : right->blocks) rights[r.first.first].push_back({r.first.second, &r.second});
-    std::map<std::pair<int32_t, int32_t>, size_t> index;
-    // left->blocks is ordered by (i, k): iterating it visits k ascending within each i
-    for (auto& l : left->blocks) {
-      const int32_t i = l.first.first, k = l.first.second;
-      auto rit = rights.find(k);
-      if (rit == rights.end()) continue;
-      for (auto& jb : rit->second) {
-        auto key = std::make_pair(i, jb.first);
-        auto it = index.find(key);
-        if (it == index.end()) {
-          OutPlan o;
-          o.rid = i;
-          o.cid = jb.first;
-          it = index.emplace(key, plans.size()).first;
-          plans.push_back(std::move(o));
-        }
-        planner.add_pair(plans[it->second], l.second, *jb.second, k);
-      }
-    }
+  const int mv = decisions ? decisions->mv : matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
+  // MatfastExecution.scala:712-713: a single block column of A and block row of B take the outer-product paths
+  const bool outer = ceil_div(leftColNum, blkSize) == 1 && ceil_div(rightRowNum, blkSize) == 1;
+  std::vector<OutPlan> plans = plan_multiply(left, right, outer, mv != MV_NONE);
+  MultiplyDecisions own;
+  if (!decisions) {
+    own = decide(ctx, plans, mv);
+    decisions = &own;
   }
-  for (OutPlan& o : plans) planner.resolve(o);
+  std::deque<Block> temps;
+  densify_operands(ctx, plans, temps);
   std::unique_ptr<mr_matrix> result(out_layout ? new_sharded(ctx, *out_layout, false, false) : new_matrix(ctx));
   if (out_layout) result->blocks.clear();  // only the blocks the product has are present (join semantics); absent ones stay absent
-  run_multiply(ctx, plans, planner, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, leftColBlkNum == 1 && rightRowBlkNum == 1,
-               out_windows, decisions, mv_side);
+  run_multiply(ctx, plans, *decisions, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, outer, out_windows);
   return result.release();
 }
 
-// The output blocks of left x right and their partial products, walked exactly as multiply_impl builds its plans (join on k in
-// ascending k, or the outer-product path with the last duplicate winning), but from metadata: no block is touched.
 MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum,
                                      const mr_matrix* right, int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
+  const int mv = matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
   MultiplyDecisions d;
-  d.mv = matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
-  if (d.mv != MV_NONE) return d;
-  using Id = std::pair<int32_t, int32_t>;
-  struct Out {
-    int32_t m = 0, n = 0;
-    bool gemm = false, other = false;
-    int64_t flops = 0, cand_flops = 0;
-    std::vector<std::pair<Id, Id>> cand;  // dense x sparse pairs that may take the route (MultiplyPlanner::resolve)
-  };
-  std::map<Id, Out> outs;
-  auto pair_into = [](Out& o, const Id& ia, const Block& a, const Id& ib, const Block& b) {
-    o.m = a.numRows;
-    o.n = b.numCols;
-    if (pair_kind(a, b) == PAIR_GEMM && dspmm_candidate(a, b)) {
-      o.cand.emplace_back(ia, ib);
-      o.cand_flops += 2ll * a.numRows * b.numCols * a.numCols;
-    } else if (pair_kind(a, b) == PAIR_GEMM) {
-      o.gemm = true;
-      o.flops += 2ll * a.numRows * b.numCols * a.numCols;
-    } else {
-      o.other = true;
-    }
-  };
-  if (ceil_div(leftColNum, blkSize) == 1 && ceil_div(rightRowNum, blkSize) == 1) {
-    for (auto& l : left->blocks)
-      for (auto& r : right->blocks) {
-        Out o;
-        pair_into(o, l.first, l.second, r.first, r.second);
-        outs[{l.first.first, r.first.second}] = o;
-      }
-  } else {
-    std::map<int32_t, std::vector<std::pair<int32_t, const Block*>>> rights;
-    for (auto& r : right->blocks) rights[r.first.first].push_back({r.first.second, &r.second});
-    for (auto& l : left->blocks) {
-      auto rit = rights.find(l.first.second);
-      if (rit == rights.end()) continue;
-      for (auto& jb : rit->second) pair_into(outs[{l.first.first, jb.first}], l.first, l.second, {l.first.second, jb.first}, *jb.second);
-    }
+  d.mv = mv;
+  if (mv != MV_NONE) return d;
+  const bool outer = ceil_div(leftColNum, blkSize) == 1 && ceil_div(rightRowNum, blkSize) == 1;
+  std::vector<OutPlan> plans;
+  try {
+    plans = plan_multiply(left, right, outer, false);
+  } catch (const MrError&) {
+    // plan_multiply raises nothing but its shape checks.  A streamed multiply reports a shape error from the tile that holds the
+    // mismatched pair, with the status and message the resident multiply of that tile gives; until then its tiles run with these
+    // default decisions (no dense x sparse scratch in the tiling bound) and their results are dropped with the error.
+    return d;
   }
-  int64_t flops = 0, tiles128 = 0;
-  bool mixed = false;
-  for (auto& kv : outs) {
-    Out& o = kv.second;
-    if (!o.cand.empty()) {
-      if (o.gemm) {  // densified next to the block's other GEMM pairs
-        o.flops += o.cand_flops;
-        for (auto& c : o.cand) d.ds_dense_right.insert(c.second);
-      } else {
-        o.other = true;
-        for (auto& c : o.cand) {
-          d.ds_left.insert(c.first);
-          d.ds_right.insert(c.second);
-        }
+  d = decide(ctx, plans, mv);
+  // the blocks of the dense x sparse pairs, for the scratch bound of the tiles
+  for (const OutPlan& o : plans)
+    for (const PlanPair& p : o.pairs)
+      if (p.route == ROUTE_DSPMM) {
+        d.ds_left.insert({o.rid, p.k});
+        d.ds_right.insert({p.kb, o.cid});
+      } else if (p.route == ROUTE_GEMM && dspmm_candidate(*p.a, *p.b)) {
+        d.ds_dense_right.insert({p.kb, o.cid});
       }
-    }
-    if (!o.gemm || o.m == 0 || o.n == 0) continue;
-    flops += o.flops;
-    tiles128 += static_cast<int64_t>((o.m + 127) / 128) * ((o.n + 127) / 128);
-    mixed = mixed || o.other;  // a block with sparse partials next to dense ones keeps the whole product off the Ozaki-II engine
-  }
-  d.variant = tiles128 >= 2 * 132 ? GEMM_128x128 : GEMM_64x64;
-  d.oz2 = !mixed && (ctx->gemm_algo == 4 || (ctx->gemm_algo == 0 && flops >= (1ll << 33)));
   return d;
 }
 
 // Upper bounds of run_dense_sparse's scratch per left block (column-major copy, non-finite sets) and right block (CSC copy of a
-// CSR block, prepared segments).
+// CSR block and its csr_to_csc cursors, prepared segments).
 size_t dspmm_left_scratch(const Block& a) {
   return align_up(static_cast<size_t>(a.numRows) * a.numCols * sizeof(double)) +
          align_up(static_cast<size_t>(a.numRows) * DS_KW * sizeof(uint32_t)) +
@@ -1842,9 +1696,7 @@ size_t dspmm_left_scratch(const Block& a) {
 }
 size_t dspmm_right_scratch(const Block& b) {
   size_t eo, ro, so, ko, n = align_up(dspmm_aux_bytes(b.numCols, b.numRows, b.valuesLen, &eo, &ro, &so, &ko));
-  if (b.isT)
-    n += align_up(static_cast<size_t>(b.numCols + 1) * sizeof(int32_t)) + align_up(static_cast<size_t>(b.valuesLen) * sizeof(int32_t)) +
-         align_up(static_cast<size_t>(b.valuesLen) * sizeof(double)) + align_up(static_cast<size_t>(b.numCols) * sizeof(int32_t));
+  if (b.isT) n += CscLayout(b.numCols, b.valuesLen).bytes + align_up(static_cast<size_t>(b.numCols) * sizeof(int32_t));
   return n;
 }
 

@@ -324,6 +324,24 @@ mr_matrix* new_matrix(mr_context* ctx);
 void validate_desc(const mr_block_desc* d);
 void check_same_dims(int64_t lr, int64_t lc, int64_t rr, int64_t rc);
 
+// The CSC copy of a CSR block (csr_to_csc): byte offsets of its arrays in a window of `bytes` bytes.
+struct CscLayout {
+  size_t ptr, idx, val, bytes;
+  CscLayout(int32_t cols, int64_t nnz);
+};
+// One CSR -> CSC conversion: the CSR arrays of a rows x cols block with nnz entries, and the window its CSC copy goes to.
+struct CsrToCsc {
+  const int32_t* ptr;
+  const int32_t* idx;
+  const double* val;
+  int32_t rows, cols;
+  int64_t nnz;
+  char* out;  // CscLayout(cols, nnz).bytes
+};
+// Runs the conversions in one launch_sptrans (indices ascending in every column; a repeated coordinate's entries end up next to
+// each other, the last stored first).  Nothing when `convs` is empty.
+void csr_to_csc(mr_context* ctx, const std::vector<CsrToCsc>& convs);
+
 // A slab allocator for operator results: one device allocation, blocks are windows into it.
 struct Slab {
   Buf buf;
