@@ -266,7 +266,7 @@ bool try_ozaki(mr_context* ctx, const std::vector<OutPlan>& plans, const std::ve
   else
     CUDA_CHECK(ozaki_gemm_f64(va.data(), static_cast<int>(va.size()), vb.data(), static_cast<int>(vb.size()), Mc, K, Nc,
                               ctx->ozaki_slices > 0 ? ctx->ozaki_slices : 7, ctab.data(), blkSize, static_cast<int>(nbr),
-                              static_cast<int>(nbc), false, &launches, &nonfinite, ctx->stream));
+                              static_cast<int>(nbc), &launches, &nonfinite, ctx->stream));
   note_launch(ctx, launches);
   if (nonfinite) return false;
   ctx->stats.gemm_launches += 1;

@@ -5,11 +5,11 @@
 //   a_ik = 2^(e_i+2) * sum_{s=1..S} A_s[i,k] * 2^(-8s)      A_s in [-128,127]  (balanced base-256 digits, |a_ik| < 2^e_i)
 //   b_kj = 2^(f_j+2) * sum_{t=1..S} B_t[k,j] * 2^(-8t)
 //   c_ij ~= sum_{d=2..S+1} 2^(e_i+f_j+4-8d) * sum_{s+t=d} (A_s B_t)_ij     (products with s+t > S+1 dropped)
-// e_i / f_j = exponent of the largest |a| in row i of A / column j of B (over ALL k-blocks), every slice
-// product is an exact s32 GEMM on the tensor cores (|digit product| <= 2^14, K*|pairs| <= 2^17 per
-// accumulator), and the only roundings are the final digit (2^-(8S-2) relative to the row/column maximum)
-// and S fp64 additions per element.  S = 7 gives errors at the level of fp64 dgemm's own rounding for
-// data of moderate dynamic range per row/column; the exact DMMA kernel (gemm_f64.cu) stays the default.
+// e_i / f_j = exponent of the largest |a| in row i of A / column j of B (over the k-blocks that meet a block of the other
+// operand), every slice product is an exact s32 GEMM on the tensor cores (|digit product| <= 2^14, K*|pairs| < 2^17 per
+// accumulator), each diagonal term is scaled by 2^(e_i+f_j+4-8d) with one rounding, and the terms are added in fp64.
+// What the result promises (the supported inputs and the element-wise bound) is DESIGN section 4.1.1; the exact DMMA
+// kernel (gemm_f64.cu) stays the default.
 //
 // Pipeline per multiply (replaces the same reference code as gemm_f64.cu: BLAS.scala:327-346,
 // MLMatrix.scala:100-104, MatfastExecutionHelper.scala:255):
@@ -98,15 +98,15 @@ __device__ __forceinline__ void wgmma_wait() {
 
 struct OzakiGemmParams {
   const unsigned char* tmaps;  // 2*S CUtensorMaps (128 B each): A_1..A_S then B_1..B_S
-  const double* row_scale;     // 2^e_i per global row of A      (|a_ik| < 2^e_i)
-  const double* col_scale;     // 2^f_j per global column of B   (|b_kj| < 2^f_j)
+  const double* row_scale;     // fp32 path: additive mean correction per global row of A
+  const double* col_scale;     // fp32 path: additive mean correction per global column of B
   double* const* ctab;         // [nbr * nbc] output block pointers (nullptr = block absent)
   int32_t M, N, Kpad;          // logical output dims, padded K (multiple of 128)
   int32_t blk, nbr, nbc;       // block size and block-grid extent of C
   int32_t S, d;                // slices, diagonal of this launch (pairs (s, d - s))
   int32_t accumulate;          // 0: C = term, 1: C += term
   int32_t tiles_m, tiles_n;    // tile grid (128 x 256 tiles)
-  double diag_scale;           // 2^(4 - 8 d)
+  const int32_t* line_exp;     // Ozaki-I: e_i per global row of A (tiles_m * BM of them), then f_j per global column of B
   // generalisation used by the fp32 path (tf32x3): explicit (A slice, B slice) tensor-map index pairs and the K extent of
   // one 128-byte stage row in elements (the accumulator type is the kernel's template parameter)
   int32_t npairs;
@@ -239,6 +239,25 @@ __device__ __forceinline__ void store_residues(const int32_t (&acc)[128], int8_t
   }
 }
 
+__device__ __forceinline__ double pow2_double(int n) {  // 2^n, -1022 <= n <= 1023
+  return __hiloint2double((n + 1023) << 20, 0);
+}
+// x 2^n rounded once, for x = 0, for an integer 1 <= |x| < 2^31 and any n, and for 2^-60 <= |x| < 2^31 and n > 1000.  The first
+// factor 2^n1 (n clamped to [-1022, 1023]) leaves |x| 2^n1 normal, so that product is exact unless it overflows -- and then n1 = 1023
+// <= n, so x 2^n overflows as well.  The second factor is 1 unless n lies outside [-1022, 1023]; then it rounds a sub-normal result
+// or overflows.  Below n = -2044 the clamp of n2 changes nothing: both the product and x 2^n round to zero.
+__device__ __forceinline__ double ldexp_int(double x, int n) {
+  const int n1 = max(-1022, min(1023, n));
+  const int n2 = max(-1022, min(1023, n - n1));
+  return __dmul_rn(__dmul_rn(x, pow2_double(n1)), pow2_double(n2));
+}
+
+// Ozaki-I terms t_d = acc_d 2^(e_i+f_j+4-8d), |acc_d| < 2^31, and their partial sums stay below 2^(e_i+f_j+20), so for
+// e_i + f_j <= OZ1_SCALED_ABOVE they are finite.  Above it they are at least 2^(e_i+f_j-60) (or zero), far from the sub-normals, so the
+// epilogue sums acc_d 2^(4-8d) instead -- the same roundings, scaled by 2^-(e_i+f_j) -- and applies 2^(e_i+f_j) once, to the sum after
+// the last diagonal (d = 2): a top-digit term above the fp64 range no longer turns a finite product into +-inf.
+constexpr int OZ1_SCALED_ABOVE = 1000;
+
 // Persistent, warp-specialised: one CTA per SM loops over the output tiles of this launch.  F32 = false: s8 operands, exact s32
 // accumulator (Ozaki slices or CRT residues); F32 = true: tf32 operands, fp32 accumulator written as is (tf32x3_gemm).
 template <bool F32>
@@ -319,11 +338,11 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
           continue;
         }
       }
-      // scale by 2^(e_i + f_j + 4 - 8d) (s32) or take as is (fp32) -> (+)= column-major fp64 output blocks
+      // scale by 2^(e_i + f_j + 4 - 8d) with one rounding (s32) or take as is (fp32) -> (+)= column-major fp64 output blocks
       // fp32 path: the fp64 mean corrections go in with the first K chunk (see slice_tf32_kernel)
       const bool f32_corr = F32 && !p.accumulate && p.row_scale != nullptr;
       bool row_ok[2];
-      int rid[2], lr[2], brows[2];
+      int rid[2], lr[2], brows[2], rexp[2];
       double rs[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -332,8 +351,10 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
         rid[h] = row_ok[h] ? row / p.blk : 0;
         lr[h] = row - rid[h] * p.blk;
         brows[h] = min(p.blk, p.M - rid[h] * p.blk);
-        rs[h] = !row_ok[h] ? 0.0 : (F32 ? (f32_corr ? p.row_scale[row] : 0.0) : p.row_scale[row] * p.diag_scale);
+        rs[h] = F32 && row_ok[h] && f32_corr ? p.row_scale[row] : 0.0;
+        rexp[h] = !F32 && row_ok[h] ? p.line_exp[row] : 0;
       }
+      const int32_t* col_exp = F32 ? nullptr : p.line_exp + p.tiles_m * BM;
       const int col0 = tn * BN + 2 * (lane & 3);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -345,10 +366,17 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
             double* blkp = p.ctab[rid[h] * p.nbc + cid];
             if (blkp != nullptr) {
               double* dst = blkp + lr[h] + static_cast<size_t>(brows[h]) * (col - cid * p.blk);
-              double term;
-              if constexpr (F32) term = static_cast<double>(acc[4 * j + e]) + (f32_corr ? rs[h] + __ldg(p.col_scale + col) : 0.0);
-              else term = (static_cast<double>(acc[4 * j + e]) * rs[h]) * __ldg(p.col_scale + col);
-              *dst = p.accumulate ? *dst + term : term;
+              if constexpr (F32) {
+                const double term = static_cast<double>(acc[4 * j + e]) + (f32_corr ? rs[h] + __ldg(p.col_scale + col) : 0.0);
+                *dst = p.accumulate ? *dst + term : term;
+              } else {
+                // the sum of an element with e_i + f_j > OZ1_SCALED_ABOVE is kept scaled by 2^-(e_i + f_j) until the last diagonal
+                const int ef = rexp[h] + __ldg(col_exp + col), k = ef > OZ1_SCALED_ABOVE ? ef : 0;
+                double v = ldexp_int(static_cast<double>(acc[4 * j + e]), ef + 4 - 8 * p.d - k);
+                if (p.accumulate) v = __dadd_rn(*dst, v);
+                if (p.d == 2 && k != 0) v = ldexp_int(v, k);
+                *dst = v;
+              }
             }
           }
         }
@@ -624,7 +652,7 @@ struct AbsmaxGrid {
 // range_bits > 0 (Ozaki-II auto-selection): also flags a line whose smallest non-zero magnitude lies more than range_bits
 // binary orders below its maximum -- such an element would keep too few of its significand bits after the per-line scaling.
 __global__ void exp_kernel(const unsigned long long* __restrict__ maxbits, const unsigned long long* __restrict__ minbits,
-                           int32_t* __restrict__ e, double* __restrict__ scale, int n, int range_bits, int* __restrict__ bad) {
+                           int32_t* __restrict__ e, int n, int range_bits, int* __restrict__ bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const double m = __longlong_as_double(static_cast<long long>(maxbits[i]));
@@ -639,7 +667,6 @@ __global__ void exp_kernel(const unsigned long long* __restrict__ maxbits, const
     }
   }
   e[i] = ex;
-  if (scale != nullptr) scale[i] = scalbn(1.0, ex);
 }
 
 // ---- pass 2: balanced base-256 digits.  out_s[line * Kpad + k], line = row of A (transpose_out = 0) or column of B --
@@ -849,9 +876,6 @@ __global__ void __launch_bounds__(256) residue_kernel(const OzBlock* __restrict_
 // scaling by 2^(e_i + f_j - 2 alpha) is a multiplication by a constructed power of two.  The tile is transposed through shared
 // memory so the stores follow the column-major output blocks.  Buffer rows / columns are organised in slots of `sstride` lines
 // (one block row / block column each); ctab[rslot * ncslots + cslot] is the output block or nullptr.
-__device__ __forceinline__ double pow2_double(int n) {  // 2^n, -1022 <= n <= 1023
-  return __hiloint2double((n + 1023) << 20, 0);
-}
 __device__ __forceinline__ double scale_by_pow2(double x, int n) {
   const int n1 = max(-1022, min(1023, n));
   x *= pow2_double(n1);
@@ -1169,8 +1193,8 @@ struct AsyncBuf {  // stream-ordered scratch
 }  // namespace
 
 cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K,
-                           int64_t N, int slices, double* const* h_ctab, int blk, int nbr, int nbc, bool accumulate,
-                           int* launches, int* nonfinite, cudaStream_t stream) {
+                           int64_t N, int slices, double* const* h_ctab, int blk, int nbr, int nbc, int* launches, int* nonfinite,
+                           cudaStream_t stream) {
   *nonfinite = 0;
   if (M <= 0 || N <= 0 || K <= 0) return cudaSuccess;
   const int S = slices < 2 ? 2 : (slices > 7 ? 7 : slices);
@@ -1189,14 +1213,13 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
     max_br = std::max(max_br, b_blocks[i].rows);
     max_bc = std::max(max_bc, b_blocks[i].cols);
   }
-  AsyncBuf d_ab(stream), d_bb(stream), d_max(stream), d_exp(stream), d_scale(stream), d_bad(stream), d_As(stream), d_Bs(stream), d_maps(stream), d_ctab(stream);
+  AsyncBuf d_ab(stream), d_bb(stream), d_max(stream), d_exp(stream), d_bad(stream), d_As(stream), d_Bs(stream), d_maps(stream), d_ctab(stream);
   OZ_CHECK(d_ab.alloc(sizeof(OzBlock) * na));
   OZ_CHECK(d_bb.alloc(sizeof(OzBlock) * nb));
   OZ_CHECK(cudaMemcpyAsync(d_ab.p, ha.data(), sizeof(OzBlock) * na, cudaMemcpyHostToDevice, stream));
   OZ_CHECK(cudaMemcpyAsync(d_bb.p, hb.data(), sizeof(OzBlock) * nb, cudaMemcpyHostToDevice, stream));
   OZ_CHECK(d_max.alloc(sizeof(unsigned long long) * (Mpad + Npad)));
   OZ_CHECK(d_exp.alloc(sizeof(int32_t) * (Mpad + Npad)));
-  OZ_CHECK(d_scale.alloc(sizeof(double) * (Mpad + Npad)));
   OZ_CHECK(d_bad.alloc(sizeof(int)));
   OZ_CHECK(cudaMemsetAsync(d_max.p, 0, sizeof(unsigned long long) * (Mpad + Npad), stream));
   OZ_CHECK(cudaMemsetAsync(d_bad.p, 0, sizeof(int), stream));
@@ -1213,8 +1236,8 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
     OZ_CHECK(for_block_chunks(nb, [&](int off, int cnt) {
       absmax_kernel<<<dim3(gb.tiles, cnt), 256, 0, stream>>>(static_cast<const OzBlock*>(d_bb.p) + off, colmax, nullptr, 0, gb.ts);
     }));
-    exp_kernel<<<static_cast<unsigned>((Mpad + Npad + 255) / 256), 256, 0, stream>>>(rowmax, nullptr, row_exp, static_cast<double*>(d_scale.p),
-                                                                                      static_cast<int>(Mpad + Npad), 0, static_cast<int*>(d_bad.p));
+    exp_kernel<<<static_cast<unsigned>((Mpad + Npad + 255) / 256), 256, 0, stream>>>(rowmax, nullptr, row_exp, static_cast<int>(Mpad + Npad), 0,
+                                                                                      static_cast<int*>(d_bad.p));
     *launches += 3;
   }
   int h_bad = 0;
@@ -1257,8 +1280,7 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
   // pass 3: smallest terms first (diagonal S+1 down to 2)
   OzakiGemmParams p{};
   p.tmaps = static_cast<const unsigned char*>(d_maps.p);
-  p.row_scale = static_cast<const double*>(d_scale.p);
-  p.col_scale = p.row_scale + Mpad;
+  p.line_exp = row_exp;  // col_exp follows at row_exp + Mpad
   p.ctab = static_cast<double* const*>(d_ctab.p);
   p.M = static_cast<int32_t>(M);
   p.N = static_cast<int32_t>(N);
@@ -1277,11 +1299,10 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t ntiles = static_cast<int64_t>(p.tiles_m) * p.tiles_n;
   const unsigned grid = static_cast<unsigned>(std::min<int64_t>(ntiles, sms));
-  bool first = !accumulate;
+  bool first = true;  // the first launch stores, the others add: the output blocks hold the (possibly scaled) partial sums
   for (int d = S + 1; d >= 2; --d) {
     p.d = d;
     p.accumulate = first ? 0 : 1;
-    p.diag_scale = std::ldexp(1.0, 4 - 8 * d);
     p.npairs = 0;
     for (int sl = std::max(1, d - S); sl <= std::min(S, d - 1); ++sl) {  // pairs (s, d - s)
       p.pair_a[p.npairs] = sl - 1;
@@ -1541,8 +1562,8 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
     e->launches += 1;
   }
   // the exponent pass flags non-finite lines only; elements too far below their line maximum are handled one by one (OutlierRec)
-  exp_kernel<<<static_cast<unsigned>((nlines + 255) / 256), 256, 0, stream>>>(e->maxb + line0, nullptr, e->exps + line0, nullptr,
-                                                                               static_cast<int>(nlines), 0, e->bad);
+  exp_kernel<<<static_cast<unsigned>((nlines + 255) / 256), 256, 0, stream>>>(e->maxb + line0, nullptr, e->exps + line0, static_cast<int>(nlines), 0,
+                                                                               e->bad);
   OZ_CHECK(cudaGetLastError());
   e->launches += 1;
   if (nblocks > 0) {
@@ -1729,7 +1750,6 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
   p.nbc = nbc;
   p.kstep = 32;
   p.accumulate = 0;
-  p.diag_scale = 1.0;
   p.row_scale = row_corr;   // fp32 path: additive mean corrections, applied with the first K chunk
   p.col_scale = col_corr;
   // small terms first: lo*hi, hi*lo, then hi*hi

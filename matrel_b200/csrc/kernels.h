@@ -78,11 +78,11 @@ struct OzakiOperand {
   uint8_t isT;
   uint8_t pad[7];
 };
-// C(blocks in h_ctab, nbr x nbc grid of blk-sized column-major blocks) (+)= A(M x K) * B(K x N); absent blocks are zeros.
+// C(blocks in h_ctab, nbr x nbc grid of blk-sized column-major blocks) = A(M x K) * B(K x N); absent blocks are zeros.
 // *nonfinite = 1 (and nothing written) when an operand holds Inf/NaN: the caller must use the exact kernel instead.
 cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K,
-                           int64_t N, int slices, double* const* h_ctab, int blk, int nbr, int nbc, bool accumulate,
-                           int* launches, int* nonfinite, cudaStream_t stream);
+                           int64_t N, int slices, double* const* h_ctab, int blk, int nbr, int nbc, int* launches,
+                           int* nonfinite, cudaStream_t stream);
 
 // Ozaki scheme II (gemm_algo 4 and the auto selection): residues modulo `moduli` pairwise-coprime p_t <= 256, one int8 tensor-core
 // GEMM per modulus, Chinese-remainder reconstruction -- as a job engine over slot-organised residue buffers (gemm_ozaki.cu).

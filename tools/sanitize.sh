@@ -10,6 +10,7 @@ run() {  # tool, tag, pytest -k expression [, test files instead of $FILES]
 }
 run memcheck dmma    "multiply_dense_vs_oracle and (131 or 300 or 40-40)"
 run memcheck ozaki   "ozaki_multiply_vs_oracle and (131 or 300)"
+run memcheck ozaki1  "irregular_shapes and (130x120x140 or 300x31x260)" tests/test_gpu_ozaki1_edges.py   # Ozaki-I: blk 50 (byte-wise digit stores), outer product with K % 4 != 0
 run memcheck crt     "crt_multiply_vs_oracle and (131 or 300 or 1024) or crt_is_bit_exact"          # engine: 1-SM (blk 64/128) and CTA-pair (blk 256) kernels
 run memcheck crtjobs "crt_pipelined or crt_panelled or corrects_isolated"           # + outlier records and the fix-up kernel                                                # pipelined groups, panelled scratch
 run memcheck crtedge "irregular_shapes and (563x563x563-blk200-sparse or 356x300x356)" tests/test_gpu_ozaki2_edges.py   # CTA pairs on ragged slots: padding tile, absent blocks
