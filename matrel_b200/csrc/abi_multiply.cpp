@@ -276,8 +276,9 @@ bool try_ozaki(mr_context* ctx, const std::vector<OutPlan>& plans, const std::ve
 
 // The largest (row panel x column panel) job grid cap_r x cap_c of an nr x nc grid of output blocks whose residue scratch fits the
 // ozaki_scratch_mb budget (0 = 16 GiB), halving the longer side first.  Returns false when not even 1 x 1 fits.  `bytes`: that
-// scratch (an upper bound of what oz2_create allocates).
-bool oz2_capacity(const mr_context* ctx, int32_t blk, int64_t K, int T, int nr, int nc, int& cap_r, int& cap_c, size_t* bytes = nullptr) {
+// scratch (an upper bound of what oz2_create allocates).  share_ab: the residues of one operand (a Gram product, nr == nc).
+bool oz2_capacity(const mr_context* ctx, int32_t blk, int64_t K, int T, int nr, int nc, int& cap_r, int& cap_c, size_t* bytes = nullptr,
+                  bool share_ab = false) {
   const int ss = (blk + kOz2TileM - 1) / kOz2TileM * kOz2TileM;
   auto panel_tiles = [&](int ncr, int ncc) {  // upper bound of a panel's tile count
     const int64_t tm = static_cast<int64_t>(ncr) * (ss / kOz2TileM);
@@ -290,13 +291,24 @@ bool oz2_capacity(const mr_context* ctx, int32_t blk, int64_t K, int T, int nr, 
   cap_c = nc;
   auto max_tiles_for = [&](int r, int cc_) { return static_cast<int>(std::min<int64_t>(plane_cap_tiles, panel_tiles(r, cc_))); };
   size_t need;
-  while ((need = oz2_scratch_bytes(blk, K, T, cap_r, cap_c, max_tiles_for(cap_r, cap_c))) > budget) {
+  while ((need = oz2_scratch_bytes(blk, K, T, cap_r, cap_c, max_tiles_for(cap_r, cap_c), share_ab)) > budget) {
     if (cap_r == 1 && cap_c == 1) return false;
     if (cap_r >= cap_c) cap_r = (cap_r + 1) / 2;
     else cap_c = (cap_c + 1) / 2;
   }
   if (bytes) *bytes = need;
   return true;
+}
+
+// The triangular tile rule of a diagonal block of a Gram product (DESIGN section 4.1.2): keep the Ozaki-II tile (a, b) of a job's
+// buffer when it holds an element (r, c) of the block with r <= c.  The block starts at buffer row row0 and column col0 and has
+// n columns.  Tiles run across slot boundaries when the slot stride is not a multiple of kOz2TileN, so the rule is applied per
+// element, block by block, and the union is kept.  With the CTA-pair kernel the caller asks for the first tile of a vertical pair,
+// so that pairs stay whole.
+bool gram_tile_kept(int a, int b, int64_t row0, int64_t col0, int n) {
+  const int64_t r_min = std::max<int64_t>(0, static_cast<int64_t>(a) * kOz2TileM - row0);
+  const int64_t c_max = std::min<int64_t>(n, static_cast<int64_t>(b + 1) * kOz2TileN - col0) - 1;
+  return r_min <= c_max;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -306,6 +318,7 @@ bool oz2_capacity(const mr_context* ctx, int32_t blk, int64_t K, int T, int nr, 
 //            block column of B that has output blocks, and turns every launch group (the chunks of a pipelined multiply, or the
 //            single group of a resident one) into jobs: which slots to prepare first, the tile list, the output-block table.
 //            Operands whose residues exceed the scratch budget are cut into (row panel x column panel) jobs that re-prepare.
+//            gram: a Gram product's blocks on and above the diagonal (gram_tile_kept); resident, its slots share their residues.
 // upload_tables(): every table goes to the device up front (before the side streams fork).
 // run_group():     enqueues the jobs of one group on a stream.  No host synchronisation anywhere: see oz2_flag().
 // ------------------------------------------------------------------------------------------------
@@ -346,7 +359,7 @@ struct Oz2Run {
   // Returns false when the multiply must stay on the exact kernel.  `group_of` may be rewritten to a single group (operands too
   // large to keep every residue resident cannot be pipelined chunk by chunk).
   bool plan(mr_context* c, const std::vector<OutPlan>& plans, const std::vector<size_t>& out_plan, const std::vector<double*>& cptr,
-            std::vector<int>& group_of, int& ngroups, int32_t blk, int64_t M, int64_t K, int64_t N, bool outer, bool guard) {
+            std::vector<int>& group_of, int& ngroups, int32_t blk, int64_t M, int64_t K, int64_t N, bool outer, bool guard, bool gram) {
     ctx = c;
     if (M <= 0 || K <= 0 || N <= 0 || K >= (1 << 17) || out_plan.empty()) return false;
     const int T = oz2_moduli_for(K, ctx->crt_moduli);
@@ -387,7 +400,11 @@ struct Oz2Run {
     }
     // ---- capacity: everything resident, or (row panel x column panel) jobs within the scratch budget
     const int64_t plane_cap_tiles = std::max<int64_t>(64, (2ll << 30) / (static_cast<int64_t>(T) * kOz2TileM * kOz2TileN));
-    if (!oz2_capacity(ctx, blk, K, T, nr, nc, cap_r, cap_c)) return false;
+    // Gram product: row slot s and column slot s hold the same block index and the same data, so they share one set of residues
+    // when every slot fits at once
+    const bool share = gram && crow == ccol && rdim == cdim && oz2_capacity(ctx, blk, K, T, nr, nc, cap_r, cap_c, nullptr, true) &&
+                       cap_r == nr && cap_c == nc;
+    if (!share && !oz2_capacity(ctx, blk, K, T, nr, nc, cap_r, cap_c)) return false;
     const bool resident = cap_r == nr && cap_c == nc;
     if (!resident) {  // panels re-prepare their slots: one group, after every operand has landed
       std::fill(group_of.begin(), group_of.end(), 0);
@@ -429,13 +446,15 @@ struct Oz2Run {
     };
     // slots that start on even 128-row tiles let the CTA-pair kernel run the tiles in vertically adjacent pairs
     const bool paired = (ss % (2 * kOz2TileM)) == 0 && ctx->force_variant != 2;
-    auto add_tiles = [&](Job& j, int rslot, int cslot, int m, int n) {
+    // diag: a diagonal block of a Gram product, whose tiles are kept only where they hold an element on or above its diagonal
+    auto add_tiles = [&](Job& j, int rslot, int cslot, int m, int n, bool diag) {
       const int tm0 = rslot * ss / kOz2TileM;
       int tm1 = (rslot * ss + m + kOz2TileM - 1) / kOz2TileM;
       if (paired && ((tm1 - tm0) & 1)) ++tm1;  // the padding tile lies inside the slot: garbage rows, never stored
       const int tn0 = cslot * ss / kOz2TileN, tn1 = (cslot * ss + n + kOz2TileN - 1) / kOz2TileN;
       for (int a = tm0; a < tm1; ++a)
-        for (int b = tn0; b < tn1; ++b) j.tiles.push_back(make_int2(a, b));
+        for (int b = tn0; b < tn1; ++b)
+          if (!diag || gram_tile_kept(paired ? a & ~1 : a, b, rslot * ss, cslot * ss, n)) j.tiles.push_back(make_int2(a, b));
     };
     auto finish_tiles = [&](Job& j) {
       std::sort(j.tiles.begin(), j.tiles.end(), [&](const int2& x, const int2& y) {
@@ -455,7 +474,8 @@ struct Oz2Run {
     };
     auto add_fix = [&](Job& j, const OutPlan& o, double* C, int rslot, int cslot) {
       if (!guard) return;
-      Oz2FixOut fo{C, o.m, o.n, rslot, cslot, static_cast<int32_t>(j.fsrcs.size()), static_cast<int32_t>(o.pairs.size())};
+      Oz2FixOut fo{C, o.m, o.n, rslot, cslot, static_cast<int32_t>(j.fsrcs.size()), static_cast<int32_t>(o.pairs.size()),
+                   gram && o.rid == o.cid ? 1 : 0, 0};
       for (const PlanPair& g : o.pairs)
         j.fsrcs.push_back(Oz2FixSrc{g.a->values.ptr<double>(), g.b->values.ptr<double>(), outer ? 0 : g.k * blk, g.a->numCols, g.a->numRows,
                                     g.b->numCols, static_cast<uint8_t>(g.a->isT), static_cast<uint8_t>(g.b->isT), {0}});
@@ -482,10 +502,20 @@ struct Oz2Run {
             newc.push_back(cc);
           }
           j.ctab[static_cast<size_t>(cr) * cap_c + cc] = cptr[out_plan[t]];
-          add_tiles(j, cr, cc, o.m, o.n);
+          add_tiles(j, cr, cc, o.m, o.n, gram && o.rid == o.cid);
           add_fix(j, o, cptr[out_plan[t]], cr, cc);
         }
         if (j.tiles.empty()) continue;
+        if (share) {  // a slot prepared on the B side is also the A slot of the same index
+          std::vector<int> ids;
+          for (int id : newr) ids.push_back(id);
+          for (int id : newc) ids.push_back(id);
+          std::sort(ids.begin(), ids.end());
+          ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
+          for (int id : ids) rprep[id] = cprep[id] = 1;
+          newr.clear();
+          newc = ids;
+        }
         for (auto& run : runs_of(newr)) j.preps.push_back(make_prep(true, run, run.front()));
         for (auto& run : runs_of(newc)) j.preps.push_back(make_prep(false, run, run.front()));
         finish_tiles(j);
@@ -509,7 +539,7 @@ struct Oz2Run {
               if (it == at.end()) continue;
               const OutPlan& o = plans[out_plan[it->second]];
               j.ctab[static_cast<size_t>(cr - r0) * cap_c + (cc - c0)] = cptr[out_plan[it->second]];
-              add_tiles(j, cr - r0, cc - c0, o.m, o.n);
+              add_tiles(j, cr - r0, cc - c0, o.m, o.n, gram && o.rid == o.cid);
               add_fix(j, o, cptr[out_plan[it->second]], cr - r0, cc - c0);
             }
           if (j.tiles.empty()) continue;
@@ -531,7 +561,7 @@ struct Oz2Run {
     if (jobs.empty()) return false;
     max_tiles = static_cast<int>(std::min<int64_t>(max_tiles, plane_cap_tiles));
     max_tiles += max_tiles & 1;
-    cudaError_t e = oz2_create(&eng, blk, K, T, cap_r, cap_c, max_tiles, guard ? 1 : 0, ctx->stream);
+    cudaError_t e = oz2_create(&eng, blk, K, T, cap_r, cap_c, max_tiles, guard ? 1 : 0, share, ctx->stream);
     if (e != cudaSuccess) {
       (void)cudaGetLastError();
       eng = nullptr;
@@ -1058,6 +1088,26 @@ int matvec_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNu
   return side;
 }
 
+// A Gram product C = A^T A or A A^T (DESIGN section 4.1.2), from block metadata: every block (k, j) of right has a block (j, k) in
+// left over the same device arrays, with swapped dims and the opposite layout flag (what mr_transpose makes), both have the same
+// number of blocks, C is square, every block is dense, and the product is not on the matrix x vector route.  gemm_algo 2 and 3
+// keep the general route.
+bool gram_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, const mr_matrix* right,
+                int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
+  if (ctx->gemm_algo != 0 && ctx->gemm_algo != 1 && ctx->gemm_algo != 4) return false;
+  if (leftRowNum != rightColNum || leftColNum != rightRowNum || left->blocks.size() != right->blocks.size()) return false;
+  for (auto& kv : right->blocks) {
+    auto it = left->blocks.find({kv.first.second, kv.first.first});
+    if (it == left->blocks.end()) return false;
+    const Block &a = it->second, &b = kv.second;
+    if (!a.dense() || !b.dense() || a.numRows != b.numCols || a.numCols != b.numRows || a.isT == b.isT) return false;
+    if (a.values.ptr<double>() != b.values.ptr<double>() || a.colPtrs.ptr<int32_t>() != b.colPtrs.ptr<int32_t>() ||
+        a.rowIndices.ptr<int32_t>() != b.rowIndices.ptr<int32_t>())
+      return false;
+  }
+  return matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize) == MV_NONE;
+}
+
 void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, bool xa) {
   std::vector<MvOut> outs;
   std::vector<MvPair> pairs;
@@ -1201,17 +1251,41 @@ std::vector<double*> allocate_outputs(mr_context* ctx, const std::vector<OutPlan
   return cptr;
 }
 
+// A Gram product's strictly-lower elements, from their transposes (gram_mirror_kernel), behind everything that writes the blocks
+// on and above the diagonal.
+void run_gram_mirror(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr) {
+  std::map<std::pair<int32_t, int32_t>, size_t> at;
+  for (size_t i = 0; i < plans.size(); ++i) at[{plans[i].rid, plans[i].cid}] = i;
+  std::vector<GramMirror> items;
+  int max_m = 0, max_n = 0;
+  for (size_t i = 0; i < plans.size(); ++i) {
+    const OutPlan& o = plans[i];
+    if (o.rid < o.cid || o.m == 0 || o.n == 0) continue;
+    const size_t up = at.at({o.cid, o.rid});
+    items.push_back(GramMirror{cptr[up], cptr[i], o.m, o.n, o.rid == o.cid ? 1 : 0, 0});
+    max_m = std::max(max_m, o.m);
+    max_n = std::max(max_n, o.n);
+    if (o.rid > o.cid) ctx->stats.gram_mirrored_blocks += 1;
+  }
+  if (items.empty()) return;
+  Buf d_items = upload(ctx, items);
+  CUDA_CHECK(launch_gram_mirror(static_cast<const GramMirror*>(d_items->p), static_cast<int>(items.size()), max_m, max_n, ctx->stream));
+  note_launch(ctx);
+}
+
 // The GEMM pairs of every output block on the dense engines: Ozaki-I / 3xTF32 (gemm_algo 2 / 3) when they fit, else ONE fused
 // DMMA launch (chunked while operands are still arriving from the host), behind the Ozaki-II engine when `dec` says to try it.
+// gram: a Gram product (DESIGN section 4.1.2), whose engines compute the blocks on and above the diagonal only; the mirror pass
+// writes the rest.
 void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, const MultiplyDecisions& dec,
-                       int32_t blkSize, mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer) {
+                       int32_t blkSize, mr_matrix* result, int64_t M, int64_t K, int64_t N, bool outer, bool gram) {
   std::vector<GemmOut> outs;
   std::vector<GemmPair> pairs;
   std::vector<size_t> out_plan;
   int64_t flops = 0;
   for (size_t i = 0; i < plans.size(); ++i) {
     const OutPlan& o = plans[i];
-    if (!o.has(ROUTE_GEMM) || o.m == 0 || o.n == 0) continue;
+    if (!o.has(ROUTE_GEMM) || o.m == 0 || o.n == 0 || (gram && o.rid > o.cid)) continue;
     GemmOut go{};
     go.C = cptr[i];
     go.m = o.m;
@@ -1236,6 +1310,7 @@ void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const
     out_plan.push_back(i);
   }
   if (outs.empty()) return;
+  if (gram) ctx->stats.gram_blocks = static_cast<int64_t>(outs.size());
   // which dense operands are still being produced on another stream (ingest copies)?
   bool pending = false;
   for (size_t i = 0; i < plans.size() && !pending; ++i)
@@ -1319,7 +1394,7 @@ void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const
   // The int8 tensor-core path (Ozaki-II residues + CRT) runs group by group in front of the DMMA launches, which then only execute
   // when the engine's device flag reports operands it cannot represent.  Small products stay on the exact kernel in auto mode.
   Oz2Run oz2;
-  const bool use_oz2 = dec.oz2 && oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0);
+  const bool use_oz2 = dec.oz2 && oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0, gram);
   auto grp = [&](const Keyed& k) { return group_of[k.t.out]; };
   std::sort(keyed.begin(), keyed.end(), [&](const Keyed& x, const Keyed& y) {
     const int gx = grp(x), gy = grp(y);
@@ -1397,7 +1472,8 @@ void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const
       for (size_t oi = 0; oi < outs.size(); ++oi)
         if (seen[oi]) {
           const OutPlan& o = plans[out_plan[oi]];
-          if (!o.has_spmm()) result->blocks[{o.rid, o.cid}].ready = r;  // blocks with sparse partials finish later
+          // blocks with sparse partials finish later, and a Gram product's diagonal blocks with the mirror pass
+          if (!o.has_spmm() && !(gram && o.rid == o.cid)) result->blocks[{o.rid, o.cid}].ready = r;
         }
     }
     t0 = t1;
@@ -1408,6 +1484,7 @@ void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const
       CUDA_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->chunk_join[i], 0));
     }
   }
+  if (gram) run_gram_mirror(ctx, plans, cptr);
   ctx->stats.gemm_launches += 1;
   ctx->stats.last_gemm_flops = flops;
   timer.stop();
@@ -1618,13 +1695,13 @@ void run_sparse_dense(mr_context* ctx, const std::vector<OutPlan>& plans, const 
 }
 
 void run_multiply(mr_context* ctx, const std::vector<OutPlan>& plans, const MultiplyDecisions& dec, int32_t blkSize, mr_matrix* result,
-                  int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows) {
+                  int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows, bool gram) {
   const std::vector<double*> cptr = allocate_outputs(ctx, plans, result, out_windows);
   if (dec.mv != MV_NONE) {
     run_matvec(ctx, plans, cptr, dec.mv == MV_XA);
     return;
   }
-  run_dense_engines(ctx, plans, cptr, dec, blkSize, result, M, K, N, outer);
+  run_dense_engines(ctx, plans, cptr, dec, blkSize, result, M, K, N, outer, gram);
   run_sparse_dense(ctx, plans, cptr);
   run_dense_sparse(ctx, plans, cptr);
   run_sparse_chains(ctx, plans, cptr, result);
@@ -1636,7 +1713,7 @@ namespace mrhost {
 
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
                          int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows,
-                         const MultiplyDecisions* decisions) {
+                         const MultiplyDecisions* decisions, bool gram) {
   for (auto& kv : left->blocks)
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
   for (auto& kv : right->blocks)
@@ -1654,7 +1731,7 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
   densify_operands(ctx, plans, temps);
   std::unique_ptr<mr_matrix> result(out_layout ? new_sharded(ctx, *out_layout, false, false) : new_matrix(ctx));
   if (out_layout) result->blocks.clear();  // only the blocks the product has are present (join semantics); absent ones stay absent
-  run_multiply(ctx, plans, *decisions, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, outer, out_windows);
+  run_multiply(ctx, plans, *decisions, blkSize, result.get(), leftRowNum, leftColNum, rightColNum, outer, out_windows, gram);
   return result.release();
 }
 
@@ -1732,10 +1809,13 @@ mr_status mr_matrix_multiply(mr_matrix* left, int64_t leftRowNum, int64_t leftCo
     ctx->stats.dspmm_products = 0;
     ctx->stats.mv_pairs = 0;
     ctx->stats.mv_sparse_entries = 0;
+    ctx->stats.gram_blocks = 0;
+    ctx->stats.gram_mirrored_blocks = 0;
     if (left->host || right->host)  // C tile by C tile through the device, into a host-resident result (abi_stream.cpp)
       *out = multiply_streamed(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
     else
-      *out = multiply_impl(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize, nullptr);
+      *out = multiply_impl(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize, nullptr, nullptr, nullptr,
+                           gram_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize));
   });
 }
 

@@ -971,16 +971,18 @@ __global__ void __launch_bounds__(256) crt_kernel(const int8_t* __restrict__ pla
 // Exact products of the outlier elements (see OutlierRec), added to the C blocks of a job after its CRT pass.  One CTA per output
 // block: first the outliers of its block row of A (C(i, :) += a_ik B(k, :), thread = column), then those of its block column of
 // B (C(:, j) += A(:, k) b_kj, thread = row; an a_ik that is an outlier itself was already paired with the original b_kj in the
-// first phase and is skipped).  Operand values come from the original fp64 blocks.
+// first phase and is skipped).  Operand values come from the original fp64 blocks.  A diagonal block of a Gram product (o.upper)
+// gets only the terms of its elements on and above the diagonal: the tiles below it may not have been stored, and the mirror
+// pass overwrites them.
 __global__ void __launch_bounds__(256) oz2_fixup_kernel(const Oz2FixOut* __restrict__ outs, const Oz2FixSrc* __restrict__ srcs,
                                                         const OutlierRec* __restrict__ recs, const int* __restrict__ rec_cnt, int cap_r,
-                                                        int sstride, const int32_t* __restrict__ row_exp, int range_bits,
+                                                        int a_slot0, int sstride, const int32_t* __restrict__ row_exp, int range_bits,
                                                         const int* __restrict__ gate) {
   if (*gate != 0) return;
   const Oz2FixOut o = outs[blockIdx.x];
-  const int nA = min(rec_cnt[o.rslot], OZ2_REC_CAP), nB = min(rec_cnt[cap_r + o.cslot], OZ2_REC_CAP);
+  const int nA = min(rec_cnt[a_slot0 + o.rslot], OZ2_REC_CAP), nB = min(rec_cnt[cap_r + o.cslot], OZ2_REC_CAP);
   if (nA == 0 && nB == 0) return;
-  const OutlierRec* ra = recs + static_cast<size_t>(o.rslot) * OZ2_REC_CAP;
+  const OutlierRec* ra = recs + static_cast<size_t>(a_slot0 + o.rslot) * OZ2_REC_CAP;
   const OutlierRec* rb = recs + static_cast<size_t>(cap_r + o.cslot) * OZ2_REC_CAP;
   for (int q = 0; q < nA; ++q) {
     const OutlierRec r = ra[q];
@@ -990,7 +992,7 @@ __global__ void __launch_bounds__(256) oz2_fixup_kernel(const Oz2FixOut* __restr
       const Oz2FixSrc sc = srcs[o.src_begin + t];
       if (r.k < sc.k0 || r.k >= sc.k0 + sc.kdim) continue;
       const int kk = r.k - sc.k0;
-      for (int j = threadIdx.x; j < o.n; j += blockDim.x) {
+      for (int j = o.upper ? i + threadIdx.x : threadIdx.x; j < o.n; j += blockDim.x) {
         const double b = sc.bT ? sc.B[static_cast<size_t>(kk) * sc.b_cols + j] : sc.B[kk + static_cast<size_t>(sc.kdim) * j];
         o.C[i + static_cast<size_t>(o.m) * j] += r.v * b;
       }
@@ -1006,7 +1008,7 @@ __global__ void __launch_bounds__(256) oz2_fixup_kernel(const Oz2FixOut* __restr
       const Oz2FixSrc sc = srcs[o.src_begin + t];
       if (r.k < sc.k0 || r.k >= sc.k0 + sc.kdim) continue;
       const int kk = r.k - sc.k0;
-      for (int i = threadIdx.x; i < o.m; i += blockDim.x) {
+      for (int i = threadIdx.x; i < (o.upper ? min(j + 1, o.m) : o.m); i += blockDim.x) {
         const double a = sc.aT ? sc.A[static_cast<size_t>(i) * sc.kdim + kk] : sc.A[i + static_cast<size_t>(sc.a_rows) * kk];
         if (a == 0.0 || exponent_of(a) < row_exp[o.rslot * sstride + i] - 1 - range_bits) continue;
         o.C[i + static_cast<size_t>(o.m) * j] += a * r.v;
@@ -1389,6 +1391,7 @@ struct Oz2Engine {
   int ksplit = 0;  // CTA-pair kernel walks (modulus, K half, tile pair) items (half the L2 footprint of the panels in flight): 1 = for
                    // long tile lists and deep K only, 2 = whenever K has an even number of chunks (tests)
   bool paired = false;   // tile lists hold vertically adjacent 128-row tiles in pairs: the CTA-pair kernel runs them
+  bool share_ab = false; // Gram product: A' is the first Mpad lines of B', and the A side reads the B side's tables (a_line0)
   int64_t K = 0, Kpad = 0, Mpad = 0, Npad = 0;
   size_t a_stride = 0, b_stride = 0, plane_stride = 0;
   int8_t *As = nullptr, *Bs = nullptr, *planes = nullptr;
@@ -1401,6 +1404,9 @@ struct Oz2Engine {
   std::vector<unsigned char> h_maps;
   int sms = 132;
   int launches = 0;
+  // where the A side's entries start in the line tables (exps) and in the slot tables (dims, recs, rec_cnt)
+  int64_t a_line0() const { return share_ab ? Mpad : 0; }
+  int a_slot0() const { return share_ab ? cap_r : 0; }
 };
 
 // K * (2^alpha)^2 <= 2^(floor(log2 P) - 1) < P / 2: the exact integer product is recovered from its residues
@@ -1426,10 +1432,10 @@ int oz2_moduli_for(int64_t K, int requested) {
   return CRT_MAX_T;
 }
 
-size_t oz2_scratch_bytes(int blk, int64_t K, int T, int cap_r, int cap_c, int max_tiles) {
+size_t oz2_scratch_bytes(int blk, int64_t K, int T, int cap_r, int cap_c, int max_tiles, bool share_ab) {
   const int64_t sstride = (blk + BM - 1) / BM * BM;
   const int64_t Kpad = (K + BKB - 1) / BKB * BKB;
-  const int64_t Mpad = sstride * cap_r, Npad = (sstride * cap_c + BN - 1) / BN * BN;
+  const int64_t Mpad = share_ab ? 0 : sstride * cap_r, Npad = (sstride * cap_c + BN - 1) / BN * BN;
   return static_cast<size_t>(T) * (Mpad + Npad) * Kpad + static_cast<size_t>(T) * max_tiles * (BM * BN);
 }
 
@@ -1440,13 +1446,14 @@ int oz2_tiles_per_block(int blk) {
 
 // Creates the engine and its scratch (stream-ordered allocations).  cap_r / cap_c = row / column slots held at once.
 cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, int guard_range,
-                       cudaStream_t stream) {
+                       bool share_ab, cudaStream_t stream) {
   *out = nullptr;
   const int T = oz2_moduli_for(K, moduli);
   int log2P[CRT_MAX_T + 1];
   OZ_CHECK(crt_constants(log2P));
   int alpha = crt_alpha(log2P[T], K);
-  if (alpha < 8 || K >= (1 << 17) || cap_r <= 0 || cap_c <= 0 || max_tiles <= 0) return cudaErrorInvalidValue;
+  if (alpha < 8 || K >= (1 << 17) || cap_r <= 0 || cap_c <= 0 || max_tiles <= 0 || (share_ab && cap_r != cap_c))
+    return cudaErrorInvalidValue;
   std::unique_ptr<Oz2Engine> e(new Oz2Engine);
   e->T = T;
   e->alpha = alpha;
@@ -1456,6 +1463,7 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
   e->cap_r = cap_r;
   e->cap_c = cap_c;
   e->max_tiles = max_tiles;
+  e->share_ab = share_ab;
   // auto mode: every non-zero element must keep >= 18 bits after the per-line scaling, which bounds the error of every product
   // term by 2^-17 of the term itself, i.e. the result by 2^-17 |A||B| element-wise (north-star tolerance 1e-5) in the worst
   // case; data of ordinary dynamic range sees the full alpha bits (1e-14 .. 1e-16)
@@ -1474,7 +1482,7 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
   auto alloc = [&](void** p, size_t n) { return cudaMallocAsync(p, n ? n : 16, stream); };
   cudaError_t err = cudaSuccess;
   const size_t lines = static_cast<size_t>(e->Mpad + e->Npad);
-  if ((err = alloc(reinterpret_cast<void**>(&e->As), e->a_stride * T)) != cudaSuccess ||
+  if ((!share_ab && (err = alloc(reinterpret_cast<void**>(&e->As), e->a_stride * T)) != cudaSuccess) ||
       (err = alloc(reinterpret_cast<void**>(&e->Bs), e->b_stride * T)) != cudaSuccess ||
       (err = alloc(reinterpret_cast<void**>(&e->planes), e->plane_stride * T)) != cudaSuccess ||
       (err = alloc(reinterpret_cast<void**>(&e->maxb), lines * 8)) != cudaSuccess ||
@@ -1494,10 +1502,12 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
     for (int t = 0; t < T; ++t)
       OZ_CHECK(cudaMemsetAsync(e->Bs + e->b_stride * t + static_cast<size_t>(e->sstride) * cap_c * e->Kpad, 0,
                                static_cast<size_t>(e->Npad - static_cast<int64_t>(e->sstride) * cap_c) * e->Kpad, stream));
-  // tensor maps: A' (box 128 rows), B' (box 256 rows: single-CTA kernel), B' (box 128 rows: each CTA of a pair loads half)
+  // tensor maps: A' (box 128 rows), B' (box 256 rows: single-CTA kernel), B' (box 128 rows: each CTA of a pair loads half).
+  // Shared residues: row slot s of A' is column slot s of B' (Mpad <= Npad)
   e->h_maps.resize(static_cast<size_t>(3 * T) * 128);
   for (int t = 0; t < T; ++t) {
-    if (!make_i8_map(&e->h_maps[static_cast<size_t>(t) * 128], e->As + e->a_stride * t, e->Kpad, e->Mpad, BM) ||
+    int8_t* a_plane = share_ab ? e->Bs + e->b_stride * t : e->As + e->a_stride * t;
+    if (!make_i8_map(&e->h_maps[static_cast<size_t>(t) * 128], a_plane, e->Kpad, e->Mpad, BM) ||
         !make_i8_map(&e->h_maps[static_cast<size_t>(T + t) * 128], e->Bs + e->b_stride * t, e->Kpad, e->Npad, BN) ||
         !make_i8_map(&e->h_maps[static_cast<size_t>(2 * T + t) * 128], e->Bs + e->b_stride * t, e->Kpad, e->Npad, BN / 2)) {
       Oz2Engine* raw = e.release();
@@ -1535,10 +1545,12 @@ int oz2_launches(Oz2Engine* e) {
 // Prepares slots [slot0, slot0 + nslots) of the A side (is_a) or B side from `nblocks` device-resident block descriptors whose
 // row0 (A) / col0 (B) already point into those slots.  d_dims = the slots' line counts (device, nslots ints).  need_zero: the
 // blocks do not cover every (line, k) of the slots (absent k-blocks, K padding): the residue rows are cleared first.
+// Shared residues (share_ab): only B slots are prepared; the A side of a slot reads the B side's residues, exponents, outlier
+// records and line counts in place.
 cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, int nblocks, int max_rows, int max_cols, int slot0,
                         int nslots, const int32_t* d_dims, bool need_zero, cudaStream_t stream) {
   if (nslots <= 0) return cudaSuccess;
-  if (slot0 < 0 || slot0 + nslots > (is_a ? e->cap_r : e->cap_c)) return cudaErrorInvalidValue;
+  if (slot0 < 0 || slot0 + nslots > (is_a ? e->cap_r : e->cap_c) || (is_a && e->share_ab)) return cudaErrorInvalidValue;
   static_assert(sizeof(OzakiOperand) == sizeof(OzBlock), "OzakiOperand is the device block descriptor");
   const OzBlock* blocks = reinterpret_cast<const OzBlock*>(d_blocks);
   const size_t line0 = (is_a ? 0 : static_cast<size_t>(e->Mpad)) + static_cast<size_t>(slot0) * e->sstride;
@@ -1638,9 +1650,9 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
       *ms_gemm += ms;
     }
     auto crt = e->crt_chunks == 3 ? crt_kernel<3> : crt_kernel<4>;
-    crt<<<static_cast<unsigned>(cnt) * 8u, 256, 0, stream>>>(e->planes, e->plane_stride, e->T, d_tiles + off, e->exps, e->exps + e->Mpad,
-                                                              2 * e->alpha, d_ctab, e->dims, e->dims + e->cap_r, e->sstride, e->cap_c,
-                                                              e->bad);
+    crt<<<static_cast<unsigned>(cnt) * 8u, 256, 0, stream>>>(e->planes, e->plane_stride, e->T, d_tiles + off, e->exps + e->a_line0(),
+                                                              e->exps + e->Mpad, 2 * e->alpha, d_ctab, e->dims + e->a_slot0(),
+                                                              e->dims + e->cap_r, e->sstride, e->cap_c, e->bad);
     OZ_CHECK(cudaGetLastError());
     e->launches += 2;
   }
@@ -1651,7 +1663,8 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
 // called behind oz2_multiply of the same job, on the same stream).  No-op for an engine without the range guard.
 cudaError_t oz2_fixup(Oz2Engine* e, const Oz2FixOut* d_outs, int nouts, const Oz2FixSrc* d_srcs, cudaStream_t stream) {
   if (nouts <= 0 || e->range_bits <= 0) return cudaSuccess;
-  oz2_fixup_kernel<<<nouts, 256, 0, stream>>>(d_outs, d_srcs, e->recs, e->rec_cnt, e->cap_r, e->sstride, e->exps, e->range_bits, e->bad);
+  oz2_fixup_kernel<<<nouts, 256, 0, stream>>>(d_outs, d_srcs, e->recs, e->rec_cnt, e->cap_r, e->a_slot0(), e->sstride, e->exps + e->a_line0(),
+                                               e->range_bits, e->bad);
   OZ_CHECK(cudaGetLastError());
   e->launches += 1;
   return cudaSuccess;

@@ -279,9 +279,10 @@ struct MultiplyDecisions {
   // blocks of the pairs densified next to GEMM pairs (the streamed multiply's scratch bound)
   std::set<std::pair<int32_t, int32_t>> ds_left, ds_right, ds_dense_right;
 };
+// gram: left x right is a Gram product (gram_route in abi_multiply.cpp, DESIGN section 4.1.2), decided by mr_matrix_multiply only
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
                          int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr,
-                         const MultiplyDecisions* decisions = nullptr);
+                         const MultiplyDecisions* decisions = nullptr, bool gram = false);
 // The decisions multiply_impl would take for left x right, from block metadata only (the blocks may be host-resident).
 MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum,
                                      const mr_matrix* right, int64_t rightRowNum, int64_t rightColNum, int32_t blkSize);

@@ -90,10 +90,12 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
 // host.  *oz2_flag() != 0 on the device means "operands not representable (Inf / NaN, or too wide a range in auto mode)": the
 // engine's remaining kernels are no-ops then and the caller's gated DMMA launch produces the blocks instead.
 struct Oz2Engine;
-size_t oz2_scratch_bytes(int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles);
+// share_ab: a Gram product (left = right^T, cap_r == cap_c): the A side of slot s is the B side of slot s, so only the B' residues
+// are held (one operand's scratch) and preparing a B slot also makes its A slot
+size_t oz2_scratch_bytes(int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, bool share_ab = false);
 int oz2_tiles_per_block(int blk);
 cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, int guard_range,
-                       cudaStream_t stream);
+                       bool share_ab, cudaStream_t stream);
 void oz2_destroy(Oz2Engine* e, cudaStream_t stream);
 const void* oz2_host_maps(const Oz2Engine* e, size_t* bytes);   // 2 * moduli CUtensorMaps to be uploaded by the caller ...
 void oz2_set_device_maps(Oz2Engine* e, const void* d_maps);     // ... and handed back as a device pointer
@@ -112,6 +114,8 @@ struct Oz2FixOut {
   int32_t m, n;
   int32_t rslot, cslot; // the engine slots its block row of A / block column of B were prepared into
   int32_t src_begin, src_count;
+  int32_t upper;        // 1: a diagonal block of a Gram product, only the elements on and above its diagonal are fixed
+  int32_t pad;
 };
 cudaError_t oz2_fixup(Oz2Engine* e, const Oz2FixOut* d_outs, int nouts, const Oz2FixSrc* d_srcs, cudaStream_t stream);
 int oz2_alpha(const Oz2Engine* e);
@@ -127,6 +131,18 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
 cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* const* d_ctab, cudaStream_t stream, double* ms_gemm,
                          cudaEvent_t ev0, cudaEvent_t ev1);
 constexpr int kOz2TileM = 128, kOz2TileN = 256;
+// Gram products C = A^T A or A A^T (gram.cu, DESIGN section 4.1.2): the engines compute the blocks on and above the diagonal;
+// ONE launch then writes dst(p, q) = src(q, p) for every strictly-lower element.  dst is m x n, src n x m, both column-major.  A
+// strictly-lower block C(i, j) has src = C(j, i); a diagonal block (diag = 1, src == dst, m == n) has only its elements below the
+// diagonal written, from the ones above it.
+struct GramMirror {
+  const double* src;
+  double* dst;
+  int32_t m, n;
+  int32_t diag, pad;
+};
+cudaError_t launch_gram_mirror(const GramMirror* d_items, int nitems, int max_m, int max_n, cudaStream_t stream);
+
 // fp32 multiply on wgmma tf32 (3xTF32 split, fp32 accumulation); same operand / output conventions.
 cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K, int64_t N,
                         double* const* h_ctab, int blk, int nbr, int nbc, int* launches, cudaStream_t stream);

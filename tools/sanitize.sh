@@ -31,3 +31,6 @@ run racecheck spmmcap "segment_capacity" tests/test_gpu_spmm_edges.py
 run racecheck crt2sm "crt_multiply_vs_oracle and 1024"
 run memcheck dspmm   "density_around_tau or nonfinite_left or repeated_coordinates or streamed_matches_resident and AB" tests/test_gpu_dspmm.py  # dense x sparse route, flag pass and fix-up
 run racecheck dspmm  "density_around_tau" tests/test_gpu_dspmm.py                 # shared-memory and global segments, empty segments skipped
+run memcheck gram    "bit_for_bit and (640 or 700) or outliers_on_both_lines or absent_blocks" tests/test_gpu_gram.py  # shared residues, triangular tiles, upper-only fix-up, mirror
+run initcheck gram   "bit_for_bit and (640 or 700) or outliers_on_both_lines" tests/test_gpu_gram.py    # nothing reads a lower element no engine stored
+run racecheck gram   "bit_for_bit and 640" tests/test_gpu_gram.py                                        # the mirror kernel's shared tile
