@@ -211,6 +211,7 @@ void compact_slots(const std::vector<OutPlan>& plans, const std::vector<size_t>&
 }
 
 // gemm_algo 2: the dense pairs of every output block through the wgmma int8 Ozaki pipeline (gemm_ozaki.cu).
+// gemm_algo 3: the same through the 3xTF32 fp32 pipeline.
 // Returns false when the problem does not fit its regular-grid assumptions or holds Inf/NaN (caller uses DMMA).
 bool try_ozaki(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, int32_t blkSize, int64_t M,
                int64_t K, int64_t N, bool outer) {
@@ -262,7 +263,7 @@ bool try_ozaki(mr_context* ctx, const std::vector<OutPlan>& plans, const std::ve
   KernelTimer timer(ctx);
   if (tf32)
     CUDA_CHECK(tf32x3_gemm(va.data(), static_cast<int>(va.size()), vb.data(), static_cast<int>(vb.size()), Mc, K, Nc, ctab.data(),
-                           blkSize, static_cast<int>(nbr), static_cast<int>(nbc), &launches, ctx->stream));
+                           blkSize, static_cast<int>(nbr), static_cast<int>(nbc), &launches, &nonfinite, ctx->stream));
   else
     CUDA_CHECK(ozaki_gemm_f64(va.data(), static_cast<int>(va.size()), vb.data(), static_cast<int>(vb.size()), Mc, K, Nc,
                               ctx->ozaki_slices > 0 ? ctx->ozaki_slices : 7, ctab.data(), blkSize, static_cast<int>(nbr),

@@ -113,6 +113,7 @@ struct OzakiGemmParams {
   int32_t pair_a[8], pair_b[8];
   int32_t kstep;               // elements of K per stage (128 int8 / 32 tf32)
   int32_t kc0, nkc;            // K range of this launch in stage units (the fp32 path re-accumulates K chunks in fp64)
+  int32_t scale_exp;           // fp32 path: the operands were scaled by 2^-sA and 2^-sB, the tile sums are scaled by 2^(sA + sB)
   // CRT mode (Ozaki scheme II, gemm_algo 4): nmod > 0 makes ONE launch walk nmod x tiles work items; item (t, tile) multiplies
   // residue matrices A mod p_t (tensor map t) and B mod p_t (tensor map nmod + t) and stores (A_t B_t) mod p_t as int8.
   int32_t nmod;
@@ -259,7 +260,7 @@ __device__ __forceinline__ double ldexp_int(double x, int n) {
 constexpr int OZ1_SCALED_ABOVE = 1000;
 
 // Persistent, warp-specialised: one CTA per SM loops over the output tiles of this launch.  F32 = false: s8 operands, exact s32
-// accumulator (Ozaki slices or CRT residues); F32 = true: tf32 operands, fp32 accumulator written as is (tf32x3_gemm).
+// accumulator (Ozaki slices or CRT residues); F32 = true: tf32 operands, fp32 accumulator scaled by 2^scale_exp (tf32x3_gemm).
 template <bool F32>
 __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const OzakiGemmParams p) {
   extern __shared__ unsigned char smem_dyn[];
@@ -367,7 +368,7 @@ __global__ void __launch_bounds__(GEMM_THREADS_P, 1) ozaki_gemm_i8_kernel(const 
             if (blkp != nullptr) {
               double* dst = blkp + lr[h] + static_cast<size_t>(brows[h]) * (col - cid * p.blk);
               if constexpr (F32) {
-                const double term = static_cast<double>(acc[4 * j + e]) + (f32_corr ? rs[h] + __ldg(p.col_scale + col) : 0.0);
+                const double term = ldexp_int(static_cast<double>(acc[4 * j + e]), p.scale_exp) + (f32_corr ? rs[h] + __ldg(p.col_scale + col) : 0.0);
                 *dst = p.accumulate ? *dst + term : term;
               } else {
                 // the sum of an element with e_i + f_j > OZ1_SCALED_ABOVE is kept scaled by 2^-(e_i + f_j) until the last diagonal
@@ -1025,34 +1026,91 @@ __device__ __forceinline__ float to_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
 }
-// Sum of all elements of the blocks (for the operand mean): the value arrays are summed in storage order (coalesced whatever
-// the block's orientation); blockIdx.x strides over 4096-element pieces, blockIdx.y = block.
-__global__ void __launch_bounds__(256) block_sum_kernel(const OzBlock* __restrict__ blocks, double* __restrict__ total) {
-  __shared__ double part[8];
+// Sum and largest |a| of the elements of one (4096-element piece, block) (the means, the scales and the Inf / NaN check; one
+// launch covers both operands, the blocks of A then those of B): the value arrays are read in storage order (coalesced whatever
+// the block's orientation); blockIdx.x strides over the pieces, blockIdx.y = block.  Each CTA writes its own slot
+// [blockIdx.y * gridDim.x + blockIdx.x] and tf32_reduce_kernel adds the slots in index order, so the sum does not depend on
+// scheduling.  The maximum is kept as the bits of |a|: NaN compares above
+// Inf, so a maximum of at least 0x7ff0... flags a non-finite operand.
+__global__ void __launch_bounds__(256) tf32_stats_kernel(const OzBlock* __restrict__ blocks, double* __restrict__ part_sum,
+                                                         unsigned long long* __restrict__ part_max) {
+  __shared__ double ps[8];
+  __shared__ unsigned long long pm[8];
   const OzBlock b = blocks[blockIdx.y];
   const size_t count = static_cast<size_t>(b.rows) * b.cols;
   double acc = 0.0;
-  for (size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x; i < count; i += static_cast<size_t>(gridDim.x) * 256) acc += b.v[i];
+  unsigned long long mx = 0;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * 256 + threadIdx.x; i < count; i += static_cast<size_t>(gridDim.x) * 256) {
+    const double v = b.v[i];
+    acc += v;
+    mx = max(mx, static_cast<unsigned long long>(__double_as_longlong(fabs(v))));
+  }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+  for (int o = 16; o > 0; o >>= 1) {
+    acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    ps[threadIdx.x >> 5] = acc;
+    pm[threadIdx.x >> 5] = mx;
+  }
   __syncthreads();
   if (threadIdx.x == 0) {
     double t = 0.0;
-    for (int w = 0; w < 8; ++w) t += part[w];
-    atomicAdd(total, t);
+    unsigned long long m = 0;
+    for (int w = 0; w < 8; ++w) {
+      t += ps[w];
+      m = max(m, pm[w]);
+    }
+    const size_t slot = static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x;
+    part_sum[slot] = t;
+    part_max[slot] = m;
   }
 }
 
-// hi = tf32(a'), lo = tf32(a' - hi) of the CENTRED fp32 value a' = fl32(a - mean): the tensor core's fp32 accumulation truncates,
-// which for same-signed data is a bias that grows with the number of accumulation steps (measured ~1e-4 at K = 16384 for U(0,1)
-// data); on centred data the same truncation errors have random signs.  The mean is put back in fp64 by the epilogue through
+// Operand totals in a fixed order: CTA x reduces the `count[x]` slots of operand x (thread t the slots t, t + 256, ..., then a
+// fixed tree), out[x] = sum, out[2 + x] = bits of the largest |a|.
+__global__ void __launch_bounds__(256) tf32_reduce_kernel(const double* __restrict__ part_sum, const unsigned long long* __restrict__ part_max,
+                                                          int64_t count_a, int64_t count_b, unsigned long long* __restrict__ out) {
+  __shared__ double ps[256];
+  __shared__ unsigned long long pm[256];
+  const int64_t first = blockIdx.x == 0 ? 0 : count_a, count = blockIdx.x == 0 ? count_a : count_b;
+  double acc = 0.0;
+  unsigned long long mx = 0;
+  for (int64_t i = threadIdx.x; i < count; i += 256) {
+    acc += part_sum[first + i];
+    mx = max(mx, part_max[first + i]);
+  }
+  ps[threadIdx.x] = acc;
+  pm[threadIdx.x] = mx;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (threadIdx.x < h) {
+      ps[threadIdx.x] += ps[threadIdx.x + h];
+      pm[threadIdx.x] = max(pm[threadIdx.x], pm[threadIdx.x + h]);
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    out[blockIdx.x] = static_cast<unsigned long long>(__double_as_longlong(ps[0]));
+    out[2 + blockIdx.x] = pm[0];
+  }
+}
+
+// hi = tf32(a'), lo = tf32(a' - hi) of the CENTRED, SCALED fp32 value a' = fl32((a - mu) 2^-s): the tensor core's fp32
+// accumulation truncates, which for same-signed data is a bias that grows with the number of accumulation steps (measured ~1e-4
+// at K = 16384 for U(0,1) data); on centred data the same truncation errors have random signs.  2^-s brings the operand's
+// largest |a| into [1, 2), so fp32 neither overflows nor loses the products to its sub-normals whatever the fp64 magnitude;
+// a' below 2^-126 (and lo below it) is flushed to zero, so the tensor core only ever sees normal numbers.  The mean is put back
+// in fp64 by the epilogue through
 //   (A' + muA 11^T)(B' + muB 11^T) = A'B' + muB (A'1) 1^T + muA 1 (1^T B') + K muA muB 11^T,
-// for which this pass also accumulates the line sums A'1 / 1^T B' (line_sum, fp64 atomics).
+// for which this pass also sums the unscaled a' 2^s of each (line, 128-k tile of a block) into its own slot
+// line_part[(kb * tiles_k_max + tk) * line_stride + line] (kb = k-block of the block); tf32_corr_kernel adds the slots in order.
 __global__ void __launch_bounds__(256) slice_tf32_kernel(const OzBlock* __restrict__ blocks, float* __restrict__ out_hi,
                                                          float* __restrict__ out_lo, int Kpad, int lines_are_rows, int tiles_k_max,
-                                                         const double* __restrict__ total, double inv_count, double* __restrict__ line_sum) {
+                                                         double mu, int s, int blk, double* __restrict__ line_part, int line_stride) {
   __shared__ double sm[32][129];
+  __shared__ double wsum[32][4];
   const OzBlock b = blocks[blockIdx.y];
   const int tl = blockIdx.x / tiles_k_max, tk = blockIdx.x % tiles_k_max;
   const int nlines = lines_are_rows ? b.rows : b.cols;
@@ -1060,7 +1118,6 @@ __global__ void __launch_bounds__(256) slice_tf32_kernel(const OzBlock* __restri
   const int l0 = tl * 32, k0 = tk * 128;
   if (l0 >= nlines || k0 >= nks) return;
   const int tid = threadIdx.x;
-  const double mu = total != nullptr ? total[0] * inv_count : 0.0;
   const bool k_fast = lines_are_rows ? (b.isT != 0) : (b.isT == 0);
   for (int idx = tid; idx < 32 * 128; idx += 256) {
     const int l = k_fast ? idx / 128 : idx % 32, k = k_fast ? idx % 128 : idx / 32;
@@ -1075,29 +1132,47 @@ __global__ void __launch_bounds__(256) slice_tf32_kernel(const OzBlock* __restri
     const int l = idx / 128, k = idx % 128;
     double contrib = 0.0;
     if (l0 + l < nlines && k0 + k < nks) {
-      const float a = static_cast<float>(sm[l][k] - mu);
+      float a = static_cast<float>(ldexp_int(sm[l][k] - mu, -s));
+      if (fabsf(a) < 0x1p-126f) a = 0.0f;
       const float hi = to_tf32(a);
-      const float lo = to_tf32(a - hi);
+      float lo = to_tf32(a - hi);
+      if (fabsf(lo) < 0x1p-126f) lo = 0.0f;
       const size_t o = static_cast<size_t>(gl_base + l) * Kpad + gk_base + k;
       out_hi[o] = hi;
       out_lo[o] = lo;
-      contrib = static_cast<double>(a);
+      contrib = ldexp_int(static_cast<double>(a), s);
     }
-    if (line_sum != nullptr) {
+    if (line_part != nullptr) {
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, o);
-      if ((tid & 31) == 0 && l0 + l < nlines) atomicAdd(&line_sum[gl_base + l], contrib);
+      if ((tid & 31) == 0) wsum[l][k >> 5] = contrib;
+    }
+  }
+  if (line_part != nullptr) {
+    __syncthreads();
+    if (tid < 32 && l0 + tid < nlines) {
+      const int kb = (lines_are_rows ? b.col0 : b.row0) / blk;
+      line_part[static_cast<size_t>(kb * tiles_k_max + tk) * line_stride + gl_base + tid] =
+          ((wsum[tid][0] + wsum[tid][1]) + wsum[tid][2]) + wsum[tid][3];
     }
   }
 }
 
-// additive fp64 corrections of the centred product: row_corr[i] = muB * (A'1)_i + K muA muB, col_corr[j] = muA * (1^T B')_j
-__global__ void tf32_corr_kernel(const double* __restrict__ totals, double inv_a, double inv_b, double K, double* __restrict__ row_corr, int m,
-                                 double* __restrict__ col_corr, int n) {
+// additive fp64 corrections of the centred product, the line sums added slot by slot in order:
+// row_corr[i] = muB * (A'1)_i + K muA muB, col_corr[j] = muA * (1^T B')_j
+__global__ void tf32_corr_kernel(const double* __restrict__ part_a, int slots_a, const double* __restrict__ part_b, int slots_b, double muA,
+                                 double muB, double K, double* __restrict__ row_corr, int m, double* __restrict__ col_corr, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const double muA = totals[0] * inv_a, muB = totals[1] * inv_b;
-  if (i < m) row_corr[i] = muB * row_corr[i] + K * muA * muB;
-  if (i < n) col_corr[i] = muA * col_corr[i];
+  if (i < m) {
+    double t = 0.0;
+    for (int q = 0; q < slots_a; ++q) t += part_a[static_cast<size_t>(q) * m + i];
+    row_corr[i] = muB * t + K * muA * muB;
+  }
+  if (i < n) {
+    double t = 0.0;
+    for (int q = 0; q < slots_b; ++q) t += part_b[static_cast<size_t>(q) * n + i];
+    col_corr[i] = muA * t;
+  }
 }
 
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1670,10 +1745,12 @@ cudaError_t oz2_fixup(Oz2Engine* e, const Oz2FixOut* d_outs, int nouts, const Oz
   return cudaSuccess;
 }
 
-// fp32 multiply on wgmma tf32 with the 3xTF32 split (gemm_algo = 3).  Inputs are rounded to fp32, products are
-// accumulated in fp32 by the tensor cores, the result is stored into the fp64 output blocks.
+// fp32 multiply on wgmma tf32 with the 3xTF32 split (gemm_algo = 3).  Operands are centred (when fully covered) and scaled by a
+// power of two, rounded to fp32, products are accumulated in fp32 by the tensor cores, the result is stored into the fp64 output
+// blocks (DESIGN section 4.3 states the error bound).  *nonfinite = 1 (and nothing written) when an operand holds Inf / NaN.
 cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K, int64_t N,
-                        double* const* h_ctab, int blk, int nbr, int nbc, int* launches, cudaStream_t stream) {
+                        double* const* h_ctab, int blk, int nbr, int nbc, int* launches, int* nonfinite, cudaStream_t stream) {
+  *nonfinite = 0;
   if (M <= 0 || N <= 0 || K <= 0) return cudaSuccess;
   const int64_t Mpad = (M + BM - 1) / BM * BM, Npad = (N + BN - 1) / BN * BN, Kpad = (K + 31) / 32 * 32;
   OZ_CHECK(configure_gemm_kernels());
@@ -1689,34 +1766,53 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
     max_br = std::max(max_br, b_blocks[i].rows);
     max_bc = std::max(max_bc, b_blocks[i].cols);
   }
-  AsyncBuf d_ab(stream), d_bb(stream), d_A(stream), d_B(stream), d_maps(stream), d_ctab(stream), d_corr(stream);
-  OZ_CHECK(d_ab.alloc(sizeof(OzBlock) * na));
-  OZ_CHECK(d_bb.alloc(sizeof(OzBlock) * nb));
-  OZ_CHECK(cudaMemcpyAsync(d_ab.p, ha.data(), sizeof(OzBlock) * na, cudaMemcpyHostToDevice, stream));
-  OZ_CHECK(cudaMemcpyAsync(d_bb.p, hb.data(), sizeof(OzBlock) * nb, cudaMemcpyHostToDevice, stream));
-  // operand means (absent blocks count as zeros: the mean is over the full M x K / K x N extent) and the correction vectors
-  OZ_CHECK(d_corr.alloc(sizeof(double) * (2 + Mpad + Npad)));
-  OZ_CHECK(cudaMemsetAsync(d_corr.p, 0, sizeof(double) * (2 + Mpad + Npad), stream));
-  double* totals = static_cast<double*>(d_corr.p);
-  double* row_corr = totals + 2;
-  double* col_corr = row_corr + Mpad;
-  const double inv_a = 1.0 / (static_cast<double>(M) * static_cast<double>(K)), inv_b = 1.0 / (static_cast<double>(K) * static_cast<double>(N));
+  AsyncBuf d_blocks(stream), d_A(stream), d_B(stream), d_maps(stream), d_ctab(stream), d_stat(stream), d_red(stream), d_corr(stream),
+      d_lines(stream);
+  // one descriptor table: the blocks of A, then those of B, so that one stats launch covers both operands
+  OZ_CHECK(d_blocks.alloc(sizeof(OzBlock) * (na + nb)));
+  const OzBlock* blocks_a = static_cast<const OzBlock*>(d_blocks.p);
+  const OzBlock* blocks_b = blocks_a + na;
+  OZ_CHECK(cudaMemcpyAsync(d_blocks.p, ha.data(), sizeof(OzBlock) * na, cudaMemcpyHostToDevice, stream));
+  OZ_CHECK(cudaMemcpyAsync(const_cast<OzBlock*>(blocks_b), hb.data(), sizeof(OzBlock) * nb, cudaMemcpyHostToDevice, stream));
+  // pass 1: sum and largest |a| of each operand, per (piece, block) slot, then added in slot order
+  const int64_t max_area = std::max(static_cast<int64_t>(max_ar) * max_ac, static_cast<int64_t>(max_br) * max_bc);
+  const int64_t pieces = std::max<int64_t>(1, std::min<int64_t>(64, (max_area + 4095) / 4096));
+  const int64_t slots_a = pieces * na, slots_b = pieces * nb;
+  OZ_CHECK(d_stat.alloc((sizeof(double) + sizeof(unsigned long long)) * (slots_a + slots_b)));
+  OZ_CHECK(d_red.alloc(4 * sizeof(unsigned long long)));
+  double* part_sum = static_cast<double*>(d_stat.p);
+  unsigned long long* part_max = reinterpret_cast<unsigned long long*>(part_sum + slots_a + slots_b);
+  OZ_CHECK(for_block_chunks(na + nb, [&](int off, int cnt) {
+    tf32_stats_kernel<<<dim3(static_cast<unsigned>(pieces), cnt), 256, 0, stream>>>(blocks_a + off, part_sum + off * pieces,
+                                                                                      part_max + off * pieces);
+  }));
+  unsigned long long* red = static_cast<unsigned long long*>(d_red.p);
+  tf32_reduce_kernel<<<2, 256, 0, stream>>>(part_sum, part_max, slots_a, slots_b, red);
+  OZ_CHECK(cudaGetLastError());
+  *launches += 2;
+  unsigned long long h_red[4];
+  OZ_CHECK(cudaMemcpyAsync(h_red, red, sizeof(h_red), cudaMemcpyDeviceToHost, stream));
+  OZ_CHECK(cudaStreamSynchronize(stream));
+  if (h_red[2] >= 0x7ff0000000000000ull || h_red[3] >= 0x7ff0000000000000ull) {
+    *nonfinite = 1;  // Inf / NaN input: it would spread to every element through the mean; the caller uses the DMMA kernel
+    return cudaSuccess;
+  }
   // centring needs A = A' + muA 11^T element for element, absent blocks (implicit zeros) included: it is applied when the
-  // blocks cover both operands completely (the dense case the fp32 configuration is about); otherwise the means stay 0
+  // blocks cover both operands completely (the dense case the fp32 configuration is about); otherwise the means stay 0.  A total
+  // beyond the fp64 range (operands near the top of it) leaves its operand uncentred: the identity holds for any mu.
   int64_t area_a = 0, area_b = 0;
   for (int i = 0; i < na; ++i) area_a += static_cast<int64_t>(a_blocks[i].rows) * a_blocks[i].cols;
   for (int i = 0; i < nb; ++i) area_b += static_cast<int64_t>(b_blocks[i].rows) * b_blocks[i].cols;
   const bool centre = area_a == M * K && area_b == K * N;
-  if (centre) {
-    const unsigned pieces_a = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(64, (static_cast<int64_t>(max_ar) * max_ac + 4095) / 4096)));
-    OZ_CHECK(for_block_chunks(na, [&](int off, int cnt) {
-      block_sum_kernel<<<dim3(pieces_a, cnt), 256, 0, stream>>>(static_cast<const OzBlock*>(d_ab.p) + off, totals);
-    }));
-    const unsigned pieces_b = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>(64, (static_cast<int64_t>(max_br) * max_bc + 4095) / 4096)));
-    OZ_CHECK(for_block_chunks(nb, [&](int off, int cnt) {
-      block_sum_kernel<<<dim3(pieces_b, cnt), 256, 0, stream>>>(static_cast<const OzBlock*>(d_bb.p) + off, totals + 1);
-    }));
-    *launches += 2;
+  double totals[2], mu[2] = {0.0, 0.0};
+  int sc[2];
+  memcpy(totals, h_red, sizeof(totals));
+  for (int x = 0; x < 2; ++x) {
+    const double inv = 1.0 / (static_cast<double>(x == 0 ? M : K) * static_cast<double>(x == 0 ? K : N));
+    if (centre && std::isfinite(totals[x] * inv)) mu[x] = totals[x] * inv;
+    double amax;
+    memcpy(&amax, &h_red[2 + x], sizeof(amax));
+    sc[x] = amax > 0.0 ? std::ilogb(amax) : 0;  // largest |a| 2^-s in [1, 2): centred values below 4
   }
   const size_t a_elems = static_cast<size_t>(Mpad) * Kpad, b_elems = static_cast<size_t>(Npad) * Kpad;
   OZ_CHECK(d_A.alloc(a_elems * 2 * sizeof(float)));
@@ -1727,22 +1823,35 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
   float* Alo = Ahi + a_elems;
   float* Bhi = static_cast<float*>(d_B.p);
   float* Blo = Bhi + b_elems;
-  {
-    const int tk = (max_ac + 127) / 128, tl = (max_ar + 31) / 32;
-    OZ_CHECK(for_block_chunks(na, [&](int off, int cnt) {
-      slice_tf32_kernel<<<dim3(tl * tk, cnt), 256, 0, stream>>>(static_cast<const OzBlock*>(d_ab.p) + off, Ahi, Alo, static_cast<int>(Kpad), 1, tk,
-                                                                centre ? totals : nullptr, inv_a, row_corr);
-    }));
-    const int tkb = (max_br + 127) / 128, tlb = (max_bc + 31) / 32;
-    OZ_CHECK(for_block_chunks(nb, [&](int off, int cnt) {
-      slice_tf32_kernel<<<dim3(tlb * tkb, cnt), 256, 0, stream>>>(static_cast<const OzBlock*>(d_bb.p) + off, Bhi, Blo, static_cast<int>(Kpad), 0, tkb,
-                                                                  centre ? totals + 1 : nullptr, inv_b, col_corr);
-    }));
+  double *row_corr = nullptr, *col_corr = nullptr, *lines_a = nullptr, *lines_b = nullptr;
+  const int tk = (max_ac + 127) / 128, tl = (max_ar + 31) / 32, tkb = (max_br + 127) / 128, tlb = (max_bc + 31) / 32;
+  const int kblocks = static_cast<int>((K + blk - 1) / blk);
+  const int lslots_a = kblocks * tk, lslots_b = kblocks * tkb;
+  if (centre) {  // line sums of the centred operands: one slot per (line, k-tile of a block), zero where no tile is
+    OZ_CHECK(d_corr.alloc(sizeof(double) * (Mpad + Npad)));
+    row_corr = static_cast<double*>(d_corr.p);
+    col_corr = row_corr + Mpad;
+    const size_t nl = static_cast<size_t>(lslots_a) * Mpad + static_cast<size_t>(lslots_b) * Npad;
+    OZ_CHECK(d_lines.alloc(sizeof(double) * nl));
+    OZ_CHECK(cudaMemsetAsync(d_lines.p, 0, sizeof(double) * nl, stream));
+    lines_a = static_cast<double*>(d_lines.p);
+    lines_b = lines_a + static_cast<size_t>(lslots_a) * Mpad;
+  }
+  OZ_CHECK(for_block_chunks(na, [&](int off, int cnt) {
+    slice_tf32_kernel<<<dim3(tl * tk, cnt), 256, 0, stream>>>(blocks_a + off, Ahi, Alo, static_cast<int>(Kpad), 1, tk,
+                                                              mu[0], sc[0], blk, lines_a, static_cast<int>(Mpad));
+  }));
+  OZ_CHECK(for_block_chunks(nb, [&](int off, int cnt) {
+    slice_tf32_kernel<<<dim3(tlb * tkb, cnt), 256, 0, stream>>>(blocks_b + off, Bhi, Blo, static_cast<int>(Kpad), 0, tkb,
+                                                                mu[1], sc[1], blk, lines_b, static_cast<int>(Npad));
+  }));
+  *launches += 2;
+  if (centre) {
     const int mx = static_cast<int>(std::max(Mpad, Npad));
-    tf32_corr_kernel<<<(mx + 255) / 256, 256, 0, stream>>>(totals, inv_a, inv_b, static_cast<double>(K), row_corr, static_cast<int>(Mpad), col_corr,
-                                                           static_cast<int>(Npad));
+    tf32_corr_kernel<<<(mx + 255) / 256, 256, 0, stream>>>(lines_a, lslots_a, lines_b, lslots_b, mu[0], mu[1], static_cast<double>(K), row_corr,
+                                                           static_cast<int>(Mpad), col_corr, static_cast<int>(Npad));
     OZ_CHECK(cudaGetLastError());
-    *launches += 3;
+    *launches += 1;
   }
   std::vector<unsigned char> hmaps(4 * 128);
   if (!make_f32_map(&hmaps[0], Ahi, Kpad, Mpad, BM) || !make_f32_map(&hmaps[128], Alo, Kpad, Mpad, BM) ||
@@ -1763,8 +1872,9 @@ cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand
   p.nbc = nbc;
   p.kstep = 32;
   p.accumulate = 0;
-  p.row_scale = row_corr;   // fp32 path: additive mean corrections, applied with the first K chunk
+  p.row_scale = row_corr;   // fp32 path: additive mean corrections (nullptr: none), applied with the first K chunk
   p.col_scale = col_corr;
+  p.scale_exp = sc[0] + sc[1];
   // small terms first: lo*hi, hi*lo, then hi*hi
   p.npairs = 3;
   p.pair_a[0] = 1; p.pair_b[0] = 2;

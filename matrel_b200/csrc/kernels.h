@@ -144,8 +144,9 @@ struct GramMirror {
 cudaError_t launch_gram_mirror(const GramMirror* d_items, int nitems, int max_m, int max_n, cudaStream_t stream);
 
 // fp32 multiply on wgmma tf32 (3xTF32 split, fp32 accumulation); same operand / output conventions.
+// *nonfinite = 1 (and nothing written) when an operand holds Inf/NaN: the caller must use the exact kernel instead.
 cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K, int64_t N,
-                        double* const* h_ctab, int blk, int nbr, int nbc, int* launches, cudaStream_t stream);
+                        double* const* h_ctab, int blk, int nbr, int nbc, int* launches, int* nonfinite, cudaStream_t stream);
 
 // ---- element-wise / layout kernels (HBM-bound), batched over blocks ---------------------------------
 enum EwOp { EW_ADD = 0, EW_MUL = 1, EW_DIV = 2, EW_RANK1 = 3, EW_RANK1_COMPAT = 4, EW_COPY = 5 };

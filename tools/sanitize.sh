@@ -15,6 +15,8 @@ run memcheck crt     "crt_multiply_vs_oracle and (131 or 300 or 1024) or crt_is_
 run memcheck crtjobs "crt_pipelined or crt_panelled or corrects_isolated"           # + outlier records and the fix-up kernel                                                # pipelined groups, panelled scratch
 run memcheck crtedge "irregular_shapes and (563x563x563-blk200-sparse or 356x300x356)" tests/test_gpu_ozaki2_edges.py   # CTA pairs on ragged slots: padding tile, absent blocks
 run memcheck tf32   "tf32x3_multiply and (300 or 512)"
+run memcheck tf32edge "exact_regime_is_bit_exact and 256x512x128 or more_than_65535_blocks" tests/test_gpu_tf32_edges.py   # stats / slice chunks, ordered reductions
+run racecheck tf32edge "exact_regime_is_bit_exact and 256x512x128" tests/test_gpu_tf32_edges.py                              # the slice pass's per-warp line sums in shared memory
 run memcheck sparse  "sparse_blocks or sparse_op_sparse or aggregates or project"
 run memcheck spsp    "sparse_times_sparse"
 run memcheck spgemm  "format_pairs_bit_exact and 0.02 or absent_and_empty or block_heights and (blk64 or blk8192) and csc_csr" tests/test_gpu_spgemm.py  # smem and global accumulators, CSR<->CSC conversion, dense and sparse fills
