@@ -413,9 +413,11 @@ typedef struct mr_stats {
                                (thin side of 1 to 8 dense columns or rows; a pair is a matrix block and a thin-side block, whatever
                                its width; summed over the tiles of a streamed multiply) */
   int64_t mv_sparse_entries; /* stored entries of the sparse blocks among those pairs */
-  int64_t gram_blocks;      /* output blocks the dense engines computed for the most recent mr_matrix_multiply when it was a Gram
-                               product (A^T A or A A^T over shared arrays: the blocks on and above the diagonal; 0 otherwise) */
-  int64_t gram_mirrored_blocks; /* strictly-lower output blocks of that product written from their transposes by the mirror pass */
+  int64_t gram_blocks;      /* output blocks computed for the most recent mr_matrix_multiply when it was a Gram product (A^T A or
+                               A A^T over shared arrays): by the dense engines, the blocks on and above the diagonal; by the sparse
+                               x sparse chains, those and the non-square blocks below it; 0 otherwise */
+  int64_t gram_mirrored_blocks; /* blocks below the diagonal of that product written from their transposes (dense: the mirror pass;
+                               sparse: square blocks, mirrored, sharing their transposes' arrays or converted from them) */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

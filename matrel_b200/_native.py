@@ -85,8 +85,8 @@ class mr_stats(C.Structure):
         ("agg_sparse_entries", C.c_int64),
         ("mv_pairs", C.c_int64),
         ("mv_sparse_entries", C.c_int64),
-        ("gram_blocks", C.c_int64),
-        ("gram_mirrored_blocks", C.c_int64),
+        ("gram_blocks", C.c_int64),           # blocks a Gram product computed (dense engines or sparse chains)
+        ("gram_mirrored_blocks", C.c_int64),  # blocks below its diagonal written from their transposes
     ]
 
 

@@ -642,10 +642,48 @@ int partial_format(bool aT, bool bT, int64_t m, int64_t n, int64_t nnz) {
   return cells <= 2 * nnz + n ? FMT_DENSE : FMT_CSC;
 }
 
-void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, mr_matrix* result) {
+// The format a chain ends in, from its per-level counts: the rules above, level by level with the layouts of o's pairs.  *nnz: the
+// entries of the final sum.
+int chain_format(const OutPlan& o, const int64_t* cp, const int64_t* cs, int64_t* nnz) {
+  int fmt = FMT_DENSE;
+  int64_t s_nnz = 0;
+  for (size_t l = 0; l < o.pairs.size(); ++l) {
+    s_nnz += cs[l];
+    const int pf = partial_format(o.pairs[l].a->isT, o.pairs[l].b->isT, o.m, o.n, cp[l]);
+    if (l == 0) fmt = pf;
+    else if (fmt == FMT_DENSE || pf == FMT_DENSE) fmt = FMT_DENSE;
+    else fmt = static_cast<int64_t>(o.m) * o.n > 2 * s_nnz + o.n + 1 ? FMT_CSC : FMT_DENSE;
+  }
+  *nnz = s_nnz;
+  return fmt;
+}
+
+// gram: the product is a sparse Gram product (gram_route, DESIGN section 4.1.2).  The chains of square blocks below the diagonal
+// are not run: each such block is its upper mirror's transpose, written after the fill (a dense window by gram_mirror_kernel,
+// sparse arrays shared with or converted from the mirror's).  Diagonal chains are triangular, and gram_sym_kernel completes their
+// sparse results.  When the count pass finds a walked line whose indices do not ascend, the mirror is not exact: every chain is
+// then run as without `gram`.
+void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, mr_matrix* result,
+                       bool gram) {
   std::vector<size_t> chains;  // empty output blocks keep the (empty) dense block allocate_outputs gave them
-  for (size_t i = 0; i < plans.size(); ++i)
-    if (plans[i].has(ROUTE_SPSP) && plans[i].m > 0 && plans[i].n > 0) chains.push_back(i);
+  std::vector<std::pair<size_t, size_t>> mirrored;  // gram: (lower plan, its chain)
+  {
+    std::map<std::pair<int32_t, int32_t>, size_t> at;
+    for (size_t i = 0; i < plans.size(); ++i) at[{plans[i].rid, plans[i].cid}] = i;
+    std::map<size_t, size_t> chain_of;
+    for (size_t i = 0; i < plans.size(); ++i) {
+      const OutPlan& o = plans[i];
+      if (!o.has(ROUTE_SPSP) || o.m <= 0 || o.n <= 0) continue;
+      if (gram && o.rid > o.cid && o.m == o.n) continue;
+      chain_of[i] = chains.size();
+      chains.push_back(i);
+    }
+    if (gram)
+      for (size_t i = 0; i < plans.size(); ++i) {
+        const OutPlan& o = plans[i];
+        if (o.has(ROUTE_SPSP) && o.m > 0 && o.rid > o.cid && o.m == o.n) mirrored.push_back({i, chain_of.at(at.at({o.cid, o.rid}))});
+      }
+  }
   if (chains.empty()) return;
   const size_t nc = chains.size();
   // ---- frames: an all-CSR chain runs as C^T = B^T A^T on the CSR arrays; any other chain in CSC, its CSR operands converted once
@@ -685,6 +723,7 @@ void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const
   int32_t count_total = 0;
   int64_t col_total = 0;
   int max_m = 0, max_levels = 0;
+  bool any_tri = false;
   for (size_t c = 0; c < nc; ++c) {
     const OutPlan& o = plans[chains[c]];
     SpgemmChain& h = ch[c];
@@ -692,8 +731,11 @@ void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const
     h.n = csr_frame[c] ? o.m : o.n;
     h.pair_begin = static_cast<int32_t>(pairs.size());
     h.levels = static_cast<int32_t>(o.pairs.size());
+    h.tri = gram && o.rid == o.cid ? 1 : 0;  // its pairs are A(i, k) x A(i, k)^T, one CSR side and one CSC side: a CSC frame
+    MR_REQUIRE(!h.tri || !csr_frame[c], MR_EINVAL, "internal: a diagonal Gram chain in the CSR frame");
+    any_tri = any_tri || h.tri;
     h.count_off = count_total;
-    count_total += 2 * h.levels;
+    count_total += (h.tri ? 4 : 2) * h.levels;
     col_total += h.n;
     max_m = std::max(max_m, h.m);
     max_levels = std::max(max_levels, h.levels);
@@ -722,12 +764,13 @@ void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const
   }
   // ---- count pass: per-level counters, scalar products, per-column counts of the final sums
   const size_t counts_off = 0, prod_off = align_up(static_cast<size_t>(count_total) * sizeof(int32_t)),
-               colcnt_off = prod_off + align_up(sizeof(unsigned long long));
+               flag_off = prod_off + align_up(sizeof(unsigned long long)), colcnt_off = flag_off + align_up(sizeof(int32_t));
   Buf meta = std::make_shared<DevBuf>(ctx, colcnt_off + static_cast<size_t>(col_total) * sizeof(int32_t));
   CUDA_CHECK(cudaMemsetAsync(meta->p, 0, colcnt_off, ctx->stream));
   char* mbase = static_cast<char*>(meta->p);
   int32_t* d_counts = reinterpret_cast<int32_t*>(mbase + counts_off);
   auto* d_products = reinterpret_cast<unsigned long long*>(mbase + prod_off);
+  int32_t* d_unsorted = reinterpret_cast<int32_t*>(mbase + flag_off);
   {
     int64_t off = 0;
     for (size_t c = 0; c < nc; ++c) {
@@ -735,57 +778,116 @@ void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const
       off += ch[c].n;
     }
   }
-  const SpgemmLaunchShape shape = spgemm_shape(max_m, max_levels);
+  const SpgemmLaunchShape shape = spgemm_shape(max_m, max_levels, any_tri);
   Buf scratch = shape.scratch_bytes ? std::make_shared<DevBuf>(ctx, shape.scratch_bytes) : nullptr;
   Buf d_pairs = upload(ctx, pairs), d_items = upload(ctx, items), d_ch = upload(ctx, ch);
   CUDA_CHECK(launch_spgemm(false, static_cast<const SpgemmItem*>(d_items->p), static_cast<int>(items.size()),
                            static_cast<const SpgemmChain*>(d_ch->p), static_cast<const SpgemmPair*>(d_pairs->p), d_counts, d_products,
-                           scratch ? scratch->p : nullptr, max_m, shape, ctx->stream));
+                           scratch ? scratch->p : nullptr, max_m, shape, gram ? d_unsorted : nullptr, ctx->stream));
   note_launch(ctx);
-  std::vector<int32_t> h_counts(static_cast<size_t>(count_total));
+  std::vector<int32_t> h_counts_v(static_cast<size_t>(count_total));
   unsigned long long h_products = 0;
-  CUDA_CHECK(cudaMemcpyAsync(h_counts.data(), d_counts, h_counts.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+  int32_t h_unsorted = 0;
+  CUDA_CHECK(cudaMemcpyAsync(h_counts_v.data(), d_counts, h_counts_v.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_CHECK(cudaMemcpyAsync(&h_products, d_products, sizeof(h_products), cudaMemcpyDeviceToHost, ctx->stream));
-  ctx->stats.d2h_bytes += static_cast<int64_t>(h_counts.size() * sizeof(int32_t) + sizeof(h_products));
+  ctx->stats.d2h_bytes += static_cast<int64_t>(h_counts_v.size() * sizeof(int32_t) + sizeof(h_products));
+  if (gram) {
+    CUDA_CHECK(cudaMemcpyAsync(&h_unsorted, d_unsorted, sizeof(h_unsorted), cudaMemcpyDeviceToHost, ctx->stream));
+    ctx->stats.d2h_bytes += static_cast<int64_t>(sizeof(h_unsorted));
+  }
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  const int32_t* h_counts = h_counts_v.data();
   ctx->stats.spgemm_pairs += static_cast<int64_t>(pairs.size());
   ctx->stats.spgemm_products += static_cast<int64_t>(h_products);
-  // ---- the reference's format rules, level by level
-  std::vector<int> fmt(nc);
-  std::vector<int64_t> nnz(nc);
-  for (size_t c = 0; c < nc; ++c) {
-    const OutPlan& o = plans[chains[c]];
-    const int32_t* cp = h_counts.data() + ch[c].count_off;
-    const int32_t* cs = cp + ch[c].levels;
-    int64_t s_nnz = 0;
-    for (int32_t l = 0; l < ch[c].levels; ++l) {
-      s_nnz += cs[l];
-      const int pf = partial_format(o.pairs[l].a->isT, o.pairs[l].b->isT, o.m, o.n, cp[l]);
-      if (l == 0) fmt[c] = pf;
-      else if (fmt[c] == FMT_DENSE || pf == FMT_DENSE) fmt[c] = FMT_DENSE;
-      else fmt[c] = static_cast<int64_t>(o.m) * o.n > 2 * s_nnz + o.n + 1 ? FMT_CSC : FMT_DENSE;
-    }
-    nnz[c] = s_nnz;
+  if (h_unsorted) {  // the mirror would not be exact: the general route
+    run_sparse_chains(ctx, plans, cptr, result, false);
+    return;
   }
-  // ---- outputs: a dense window (the caller's, or from a slab of the dense-ending chains), or exactly sized sparse arrays
-  size_t dense_total = 0, sparse_total = 0;
+  // ---- the reference's format rules, level by level; a triangular chain's full counts are 2 upper - diagonal
+  std::vector<int> fmt(nc);
+  std::vector<int64_t> nnz(nc), nnz_up(nc);
+  std::vector<std::vector<int64_t>> cnt_p(nc), cnt_s(nc);
+  for (size_t c = 0; c < nc; ++c) {
+    const int32_t L = ch[c].levels;
+    const int32_t* cu = h_counts + ch[c].count_off;
+    cnt_p[c].resize(L);
+    cnt_s[c].resize(L);
+    int64_t up = 0;
+    for (int32_t l = 0; l < L; ++l) {
+      up += cu[L + l];
+      cnt_p[c][l] = ch[c].tri ? 2ll * cu[l] - cu[2 * L + l] : cu[l];
+      cnt_s[c][l] = ch[c].tri ? 2ll * cu[L + l] - cu[3 * L + l] : cu[L + l];
+    }
+    nnz_up[c] = up;
+    fmt[c] = chain_format(plans[chains[c]], cnt_p[c].data(), cnt_s[c].data(), &nnz[c]);
+    MR_REQUIRE(!ch[c].tri || fmt[c] != FMT_CSR, MR_EINVAL, "internal: a diagonal Gram chain ending CSR");
+  }
+  // a mirrored block: its own pairs' layouts and its mirror's counts (nnz(P_l), nnz(S_l) do not change under transposition).  The
+  // rules' thresholds of a square block pair up, so both end dense or both sparse; a CSR result only comes from a CSC frame.
+  std::vector<int> mfmt(mirrored.size());
+  for (size_t t = 0; t < mirrored.size(); ++t) {
+    const size_t c = mirrored[t].second;
+    int64_t e = 0;
+    mfmt[t] = chain_format(plans[mirrored[t].first], cnt_p[c].data(), cnt_s[c].data(), &e);
+    MR_REQUIRE((mfmt[t] == FMT_DENSE) == (fmt[c] == FMT_DENSE) && e == nnz[c] && !(mfmt[t] == FMT_CSR && csr_frame[c]), MR_EINVAL,
+               "internal: a Gram block and its mirror disagree on their format");
+  }
+  // ---- outputs: a dense window (the caller's, or from a slab of the dense-ending chains), or exactly sized sparse arrays.  A
+  // triangular chain's sparse upper triangle and its transpose go to `tmp`, freed behind the launches.
+  size_t dense_total = 0, sparse_total = 0, tmp_total = 0;
+  auto sparse_bytes = [](int32_t lines, int64_t e) {
+    return align_up((static_cast<size_t>(lines) + 1) * sizeof(int32_t)) + align_up(static_cast<size_t>(e) * sizeof(int32_t)) +
+           align_up(static_cast<size_t>(e) * sizeof(double));
+  };
   for (size_t c = 0; c < nc; ++c) {
     const OutPlan& o = plans[chains[c]];
     if (fmt[c] == FMT_DENSE) {
       if (!cptr[chains[c]]) dense_total += align_up(static_cast<size_t>(o.m) * o.n * sizeof(double));
     } else {
-      const bool via_csr = csr_frame[c] && fmt[c] == FMT_CSC;  // S in the CSR frame, converted to CSC at the end
-      const size_t e = static_cast<size_t>(nnz[c]);
-      sparse_total += align_up((static_cast<size_t>(ch[c].n) + 1) * sizeof(int32_t)) + align_up(e * sizeof(int32_t)) +
-                      align_up(e * sizeof(double));
-      if (via_csr) sparse_total += CscLayout(o.n, nnz[c]).bytes;
+      sparse_total += sparse_bytes(ch[c].n, nnz[c]);
+      if (csr_frame[c] && fmt[c] == FMT_CSC) sparse_total += CscLayout(o.n, nnz[c]).bytes;  // S in the CSR frame, then CSC
+      if (ch[c].tri) tmp_total += sparse_bytes(ch[c].n, nnz_up[c]) + CscLayout(o.n, nnz_up[c]).bytes + align_up(o.n * sizeof(int32_t));
     }
   }
-  std::unique_ptr<Slab> dslab, sslab;
+  for (size_t t = 0; t < mirrored.size(); ++t) {
+    const OutPlan& o = plans[mirrored[t].first];
+    const size_t c = mirrored[t].second;
+    if (mfmt[t] == FMT_DENSE) {
+      if (!cptr[mirrored[t].first]) dense_total += align_up(static_cast<size_t>(o.m) * o.n * sizeof(double));
+    } else if (mfmt[t] == FMT_CSC && !csr_frame[c]) {
+      sparse_total += CscLayout(o.n, nnz[c]).bytes;
+    }
+  }
+  std::unique_ptr<Slab> dslab, sslab, tslab;
   if (dense_total) dslab.reset(new Slab(ctx, dense_total));
   if (sparse_total) sslab.reset(new Slab(ctx, sparse_total));
+  if (tmp_total) tslab.reset(new Slab(ctx, tmp_total));
   std::vector<ScanDesc> scans;
   std::vector<CsrToCsc> finals;
+  std::vector<GramMirror> mirrors;
+  std::vector<GramSym> syms;
+  std::vector<ScanDesc> sym_scans;
+  std::vector<Span> frame_ptr(nc), frame_idx(nc), frame_val(nc);  // a sparse chain's arrays in its frame
+  int mir_m = 0, mir_n = 0, sym_n = 0;
+  auto sparse_block = [](int32_t m, int32_t n, int64_t e, bool isT, Span ptr, Span idx, Span val) {
+    Block b;
+    b.type = 0;
+    b.numRows = m;
+    b.numCols = n;
+    b.valuesLen = e;
+    b.colPtrs = ptr;
+    b.rowIndices = idx;
+    b.values = val;
+    b.colPtrsLen = (isT ? m : n) + 1;
+    b.isT = isT;
+    return b;
+  };
+  auto csc_window = [](const Span& w, int32_t cols, int64_t e, Span& ptr, Span& idx, Span& val) {
+    const CscLayout L(cols, e);
+    ptr = Span{w.buf, w.off + L.ptr};
+    idx = Span{w.buf, w.off + L.idx};
+    val = Span{w.buf, w.off + L.val};
+  };
   for (size_t c = 0; c < nc; ++c) {
     const OutPlan& o = plans[chains[c]];
     SpgemmChain& h = ch[c];
@@ -800,37 +902,83 @@ void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const
       }
       h.drs = csr_frame[c] ? o.m : 1;
       h.dcs = csr_frame[c] ? 1 : o.m;
+      if (h.tri) {
+        mirrors.push_back(GramMirror{h.dense, h.dense, o.m, o.n, 1, 0});
+        mir_m = std::max(mir_m, o.m);
+        mir_n = std::max(mir_n, o.n);
+      }
       continue;
     }
     const size_t e = static_cast<size_t>(nnz[c]);
     Span ptr = sslab->take((static_cast<size_t>(h.n) + 1) * sizeof(int32_t)), idx = sslab->take(e * sizeof(int32_t)),
          val = sslab->take(e * sizeof(double));
+    frame_ptr[c] = ptr;
+    frame_idx[c] = idx;
+    frame_val[c] = val;
+    if (h.tri) {  // the fill writes U to tmp; U^T, then the full columns into ptr / idx / val
+      const size_t eu = static_cast<size_t>(nnz_up[c]);
+      Span uptr = tslab->take((static_cast<size_t>(h.n) + 1) * sizeof(int32_t)), uidx = tslab->take(eu * sizeof(int32_t)),
+           uval = tslab->take(eu * sizeof(double)), tw = tslab->take(CscLayout(h.n, nnz_up[c]).bytes),
+           cnt = tslab->take(static_cast<size_t>(h.n) * sizeof(int32_t));
+      h.optr = uptr.ptr<int32_t>();
+      h.oidx = uidx.ptr<int32_t>();
+      h.oval = uval.ptr<double>();
+      scans.push_back(ScanDesc{h.colcnt, uptr.ptr<int32_t>(), h.n, 0});
+      // U's CSC arrays are the CSR arrays of U^T: their CSC copy is U^T's CSC
+      finals.push_back(CsrToCsc{uptr.ptr<int32_t>(), uidx.ptr<int32_t>(), uval.ptr<double>(), h.n, h.m, nnz_up[c], tw.ptr<char>()});
+      Span tp, ti, tv;
+      csc_window(tw, h.m, nnz_up[c], tp, ti, tv);
+      syms.push_back(GramSym{uptr.ptr<int32_t>(), uidx.ptr<int32_t>(), uval.ptr<double>(), tp.ptr<int32_t>(), ti.ptr<int32_t>(),
+                             tv.ptr<double>(), cnt.ptr<int32_t>(), ptr.ptr<int32_t>(), idx.ptr<int32_t>(), val.ptr<double>(), h.n, 0});
+      sym_scans.push_back(ScanDesc{cnt.ptr<int32_t>(), ptr.ptr<int32_t>(), h.n, 0});
+      sym_n = std::max(sym_n, h.n);
+      out = sparse_block(o.m, o.n, static_cast<int64_t>(e), false, ptr, idx, val);
+      continue;
+    }
     h.optr = ptr.ptr<int32_t>();
     h.oidx = idx.ptr<int32_t>();
     h.oval = val.ptr<double>();
     scans.push_back(ScanDesc{h.colcnt, ptr.ptr<int32_t>(), h.n, 0});
-    Block b;
-    b.type = 0;
-    b.numRows = o.m;
-    b.numCols = o.n;
-    b.valuesLen = static_cast<int64_t>(e);
     if (csr_frame[c] && fmt[c] == FMT_CSC) {  // CSR arrays of C -> CSC
-      const CscLayout L(o.n, b.valuesLen);
-      const Span w = sslab->take(L.bytes);
-      finals.push_back(CsrToCsc{ptr.ptr<int32_t>(), idx.ptr<int32_t>(), val.ptr<double>(), o.m, o.n, b.valuesLen, w.ptr<char>()});
-      b.colPtrs = Span{w.buf, w.off + L.ptr};
-      b.rowIndices = Span{w.buf, w.off + L.idx};
-      b.values = Span{w.buf, w.off + L.val};
-      b.colPtrsLen = o.n + 1;
-      b.isT = false;
+      const Span w = sslab->take(CscLayout(o.n, nnz[c]).bytes);
+      finals.push_back(CsrToCsc{ptr.ptr<int32_t>(), idx.ptr<int32_t>(), val.ptr<double>(), o.m, o.n, nnz[c], w.ptr<char>()});
+      Span p2, i2, v2;
+      csc_window(w, o.n, nnz[c], p2, i2, v2);
+      out = sparse_block(o.m, o.n, nnz[c], false, p2, i2, v2);
     } else {  // the frame's arrays are the result's: CSC (CSC frame) or CSR (CSR frame)
-      b.colPtrs = ptr;
-      b.rowIndices = idx;
-      b.values = val;
-      b.colPtrsLen = h.n + 1;
-      b.isT = csr_frame[c] != 0;
+      out = sparse_block(o.m, o.n, nnz[c], csr_frame[c] != 0, ptr, idx, val);
     }
-    out = std::move(b);
+  }
+  // ---- mirrored blocks.  The frame arrays of the mirror are the CSR (CSC frame) or CSC (CSR frame) arrays of this block: its
+  // result when that is its format (the arrays are shared, as A.t() shares A's), else converted to CSC.
+  for (size_t t = 0; t < mirrored.size(); ++t) {
+    const OutPlan& o = plans[mirrored[t].first];
+    const size_t c = mirrored[t].second;
+    Block& out = result->blocks[{o.rid, o.cid}];
+    if (mfmt[t] == FMT_DENSE) {
+      double* dst = cptr[mirrored[t].first];
+      if (!dst) {
+        Span s = dslab->take(static_cast<size_t>(o.m) * o.n * sizeof(double));
+        dst = s.ptr<double>();
+        out = dense_block(o.m, o.n, s, false);
+      }
+      mirrors.push_back(GramMirror{ch[c].dense, dst, o.m, o.n, 0, 0});
+      mir_m = std::max(mir_m, o.m);
+      mir_n = std::max(mir_n, o.n);
+    } else if (mfmt[t] == FMT_CSC && !csr_frame[c]) {
+      const Span w = sslab->take(CscLayout(o.n, nnz[c]).bytes);
+      finals.push_back(CsrToCsc{frame_ptr[c].ptr<int32_t>(), frame_idx[c].ptr<int32_t>(), frame_val[c].ptr<double>(), o.m, o.n, nnz[c],
+                                w.ptr<char>()});
+      Span p2, i2, v2;
+      csc_window(w, o.n, nnz[c], p2, i2, v2);
+      out = sparse_block(o.m, o.n, nnz[c], false, p2, i2, v2);
+    } else {
+      out = sparse_block(o.m, o.n, nnz[c], mfmt[t] == FMT_CSR, frame_ptr[c], frame_idx[c], frame_val[c]);
+    }
+  }
+  if (gram) {
+    ctx->stats.gram_blocks += static_cast<int64_t>(nc);
+    ctx->stats.gram_mirrored_blocks += static_cast<int64_t>(mirrored.size());
   }
   // ---- fill pass
   if (!scans.empty()) {
@@ -841,9 +989,22 @@ void run_sparse_chains(mr_context* ctx, const std::vector<OutPlan>& plans, const
   Buf d_ch2 = upload(ctx, ch);
   CUDA_CHECK(launch_spgemm(true, static_cast<const SpgemmItem*>(d_items->p), static_cast<int>(items.size()),
                            static_cast<const SpgemmChain*>(d_ch2->p), static_cast<const SpgemmPair*>(d_pairs->p), d_counts, d_products,
-                           scratch ? scratch->p : nullptr, max_m, shape, ctx->stream));
+                           scratch ? scratch->p : nullptr, max_m, shape, nullptr, ctx->stream));
   note_launch(ctx);
   csr_to_csc(ctx, finals);
+  if (!syms.empty()) {
+    Buf d_syms = upload(ctx, syms), d_sym_scans = upload(ctx, sym_scans);
+    CUDA_CHECK(launch_gram_sym(false, static_cast<const GramSym*>(d_syms->p), static_cast<int>(syms.size()), sym_n, ctx->stream));
+    CUDA_CHECK(launch_exclusive_scan(static_cast<const ScanDesc*>(d_sym_scans->p), static_cast<int>(sym_scans.size()), ctx->stream));
+    CUDA_CHECK(launch_gram_sym(true, static_cast<const GramSym*>(d_syms->p), static_cast<int>(syms.size()), sym_n, ctx->stream));
+    note_launch(ctx, 3);
+  }
+  if (!mirrors.empty()) {
+    Buf d_mirrors = upload(ctx, mirrors);
+    CUDA_CHECK(launch_gram_mirror(static_cast<const GramMirror*>(d_mirrors->p), static_cast<int>(mirrors.size()), mir_m, mir_n,
+                                  ctx->stream));
+    note_launch(ctx);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1091,22 +1252,27 @@ int matvec_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNu
 
 // A Gram product C = A^T A or A A^T (DESIGN section 4.1.2), from block metadata: every block (k, j) of right has a block (j, k) in
 // left over the same device arrays, with swapped dims and the opposite layout flag (what mr_transpose makes), both have the same
-// number of blocks, C is square, every block is dense, and the product is not on the matrix x vector route.  gemm_algo 2 and 3
-// keep the general route.
-bool gram_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, const mr_matrix* right,
-                int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
-  if (ctx->gemm_algo != 0 && ctx->gemm_algo != 1 && ctx->gemm_algo != 4) return false;
-  if (leftRowNum != rightColNum || leftColNum != rightRowNum || left->blocks.size() != right->blocks.size()) return false;
+// number of blocks, C is square, and the product is not on the matrix x vector route.  Then GRAM_DENSE when every block is dense
+// and gemm_algo is 0, 1 or 4 (2 and 3 keep the general route); GRAM_SPARSE when every block is sparse, under any gemm_algo (the
+// sparse x sparse chains do not depend on it), and multiply_impl keeps it only when every output block is a chain.
+GramKind gram_route(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, const mr_matrix* right,
+                    int64_t rightRowNum, int64_t rightColNum, int32_t blkSize) {
+  if (leftRowNum != rightColNum || leftColNum != rightRowNum || left->blocks.size() != right->blocks.size()) return GRAM_NONE;
+  size_t ndense = 0;
   for (auto& kv : right->blocks) {
     auto it = left->blocks.find({kv.first.second, kv.first.first});
-    if (it == left->blocks.end()) return false;
+    if (it == left->blocks.end()) return GRAM_NONE;
     const Block &a = it->second, &b = kv.second;
-    if (!a.dense() || !b.dense() || a.numRows != b.numCols || a.numCols != b.numRows || a.isT == b.isT) return false;
+    if (a.dense() != b.dense() || a.numRows != b.numCols || a.numCols != b.numRows || a.isT == b.isT) return GRAM_NONE;
     if (a.values.ptr<double>() != b.values.ptr<double>() || a.colPtrs.ptr<int32_t>() != b.colPtrs.ptr<int32_t>() ||
         a.rowIndices.ptr<int32_t>() != b.rowIndices.ptr<int32_t>())
-      return false;
+      return GRAM_NONE;
+    ndense += a.dense() ? 1 : 0;
   }
-  return matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize) == MV_NONE;
+  if (matvec_route(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize) != MV_NONE) return GRAM_NONE;
+  if (ndense == 0) return GRAM_SPARSE;
+  if (ndense < right->blocks.size()) return GRAM_NONE;  // mixed: pairs (i, j) and (j, i) take different kernels
+  return ctx->gemm_algo == 0 || ctx->gemm_algo == 1 || ctx->gemm_algo == 4 ? GRAM_DENSE : GRAM_NONE;
 }
 
 void run_matvec(mr_context* ctx, const std::vector<OutPlan>& plans, const std::vector<double*>& cptr, bool xa) {
@@ -1696,16 +1862,16 @@ void run_sparse_dense(mr_context* ctx, const std::vector<OutPlan>& plans, const 
 }
 
 void run_multiply(mr_context* ctx, const std::vector<OutPlan>& plans, const MultiplyDecisions& dec, int32_t blkSize, mr_matrix* result,
-                  int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows, bool gram) {
+                  int64_t M, int64_t K, int64_t N, bool outer, const OutWindowFn* out_windows, GramKind gram) {
   const std::vector<double*> cptr = allocate_outputs(ctx, plans, result, out_windows);
   if (dec.mv != MV_NONE) {
     run_matvec(ctx, plans, cptr, dec.mv == MV_XA);
     return;
   }
-  run_dense_engines(ctx, plans, cptr, dec, blkSize, result, M, K, N, outer, gram);
+  run_dense_engines(ctx, plans, cptr, dec, blkSize, result, M, K, N, outer, gram == GRAM_DENSE);
   run_sparse_dense(ctx, plans, cptr);
   run_dense_sparse(ctx, plans, cptr);
-  run_sparse_chains(ctx, plans, cptr, result);
+  run_sparse_chains(ctx, plans, cptr, result, gram == GRAM_SPARSE);
 }
 
 }  // namespace
@@ -1714,7 +1880,7 @@ namespace mrhost {
 
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
                          int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows,
-                         const MultiplyDecisions* decisions, bool gram) {
+                         const MultiplyDecisions* decisions, GramKind gram) {
   for (auto& kv : left->blocks)
     if (!kv.second.dense()) wait_ready(ctx, kv.second);
   for (auto& kv : right->blocks)
@@ -1723,6 +1889,9 @@ mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, i
   // MatfastExecution.scala:712-713: a single block column of A and block row of B take the outer-product paths
   const bool outer = ceil_div(leftColNum, blkSize) == 1 && ceil_div(rightRowNum, blkSize) == 1;
   std::vector<OutPlan> plans = plan_multiply(left, right, outer, mv != MV_NONE);
+  // a sparse Gram product whose output blocks are all chains (every pair at density <= 0.1 on both sides)
+  if (gram == GRAM_SPARSE && !std::all_of(plans.begin(), plans.end(), [](const OutPlan& o) { return o.only(ROUTE_SPSP); }))
+    gram = GRAM_NONE;
   MultiplyDecisions own;
   if (!decisions) {
     own = decide(ctx, plans, mv);

@@ -6,6 +6,10 @@
 // sides are coalesced.  Tiles are addressed within an item as (tile row, tile column), grid-strided by blockIdx.x; items by
 // blockIdx.y.  A diagonal item skips the tiles wholly above its diagonal and, in the tiles it crosses, reads only the elements
 // strictly above it and writes only those strictly below it: the engines may not have stored anything below.
+//
+// gram_sym_kernel: the sparse counterpart for a diagonal block of a sparse Gram product, whose chain produced its upper triangle U
+// only (spgemm.cu, triangular chains).  One warp per column c of the full block: U(:, c) (rows <= c), then U^T(:, c) past its
+// diagonal entry (rows > c).  Both segments ascend, so the column does too.
 #include "kernels.h"
 
 namespace matrel {
@@ -40,7 +44,50 @@ __global__ void __launch_bounds__(kMirTile * kMirRows) gram_mirror_kernel(const 
   }
 }
 
+// diagonal entry of column c present in U (its last entry, rows ascending)
+__device__ __forceinline__ int gram_sym_diag(const GramSym& g, int c) {
+  const int e = g.up[c + 1];
+  return e > g.up[c] && g.ui[e - 1] == c ? 1 : 0;
+}
+
+constexpr int kSymWarps = 8;
+
+template <bool FILL>
+__global__ void __launch_bounds__(kSymWarps * 32) gram_sym_kernel(const GramSym* __restrict__ items) {
+  const GramSym g = items[blockIdx.y];
+  const int lane = threadIdx.x & 31;
+  for (int c = blockIdx.x * kSymWarps + (threadIdx.x >> 5); c < g.n; c += gridDim.x * kSymWarps) {
+    const int u0 = g.up[c], u1 = g.up[c + 1];
+    const int t0 = g.tp[c] + gram_sym_diag(g, c), t1 = g.tp[c + 1];
+    if (!FILL) {
+      if (lane == 0) g.cnt[c] = (u1 - u0) + (t1 - t0);
+      continue;
+    }
+    const int o = g.optr[c];
+    for (int e = u0 + lane; e < u1; e += 32) {
+      g.oidx[o + e - u0] = g.ui[e];
+      g.oval[o + e - u0] = g.uv[e];
+    }
+    const int o2 = o + (u1 - u0);
+    for (int e = t0 + lane; e < t1; e += 32) {
+      g.oidx[o2 + e - t0] = g.ti[e];
+      g.oval[o2 + e - t0] = g.tv[e];
+    }
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_gram_sym(bool fill, const GramSym* d_items, int nitems, int max_n, cudaStream_t stream) {
+  if (nitems <= 0 || max_n <= 0) return cudaSuccess;
+  const int bx = std::min((max_n + kSymWarps - 1) / kSymWarps, 1024);
+  for (int off = 0; off < nitems; off += 65535) {
+    const dim3 grid(bx, std::min(nitems - off, 65535));
+    if (fill) gram_sym_kernel<true><<<grid, kSymWarps * 32, 0, stream>>>(d_items + off);
+    else gram_sym_kernel<false><<<grid, kSymWarps * 32, 0, stream>>>(d_items + off);
+  }
+  return cudaGetLastError();
+}
 
 cudaError_t launch_gram_mirror(const GramMirror* d_items, int nitems, int max_m, int max_n, cudaStream_t stream) {
   if (nitems <= 0 || max_m <= 0 || max_n <= 0) return cudaSuccess;

@@ -279,10 +279,12 @@ struct MultiplyDecisions {
   // blocks of the pairs densified next to GEMM pairs (the streamed multiply's scratch bound)
   std::set<std::pair<int32_t, int32_t>> ds_left, ds_right, ds_dense_right;
 };
-// gram: left x right is a Gram product (gram_route in abi_multiply.cpp, DESIGN section 4.1.2), decided by mr_matrix_multiply only
+// gram: left x right is a Gram product (gram_route in abi_multiply.cpp, DESIGN section 4.1.2), decided by mr_matrix_multiply only:
+// every block dense (the dense engines), or every block sparse (the sparse x sparse chains, when every output block is one).
+enum GramKind { GRAM_NONE = 0, GRAM_DENSE = 1, GRAM_SPARSE = 2 };
 mr_matrix* multiply_impl(mr_context* ctx, mr_matrix* left, int64_t leftRowNum, int64_t leftColNum, mr_matrix* right, int64_t rightRowNum,
                          int64_t rightColNum, int32_t blkSize, const ShardLayout* out_layout, const OutWindowFn* out_windows = nullptr,
-                         const MultiplyDecisions* decisions = nullptr, bool gram = false);
+                         const MultiplyDecisions* decisions = nullptr, GramKind gram = GRAM_NONE);
 // The decisions multiply_impl would take for left x right, from block metadata only (the blocks may be host-resident).
 MultiplyDecisions multiply_decisions(const mr_context* ctx, const mr_matrix* left, int64_t leftRowNum, int64_t leftColNum,
                                      const mr_matrix* right, int64_t rightRowNum, int64_t rightColNum, int32_t blkSize);

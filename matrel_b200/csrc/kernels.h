@@ -143,6 +143,24 @@ struct GramMirror {
 };
 cudaError_t launch_gram_mirror(const GramMirror* d_items, int nitems, int max_m, int max_n, cudaStream_t stream);
 
+// A symmetric n x n CSC block from its upper triangle U (CSC, rows <= column, ascending) and U^T (CSC, ascending): column c is
+// U(:, c) followed by the entries of U^T(:, c) below the diagonal.  fill = false: cnt[c] = the column's entries (then
+// launch_exclusive_scan makes optr); fill = true: writes oidx / oval at optr.
+struct GramSym {
+  const int32_t* up;
+  const int32_t* ui;
+  const double* uv;
+  const int32_t* tp;
+  const int32_t* ti;
+  const double* tv;
+  int32_t* cnt;
+  const int32_t* optr;
+  int32_t* oidx;
+  double* oval;
+  int32_t n;
+  int32_t pad;
+};
+cudaError_t launch_gram_sym(bool fill, const GramSym* d_items, int nitems, int max_n, cudaStream_t stream);
 // fp32 multiply on wgmma tf32 (3xTF32 split, fp32 accumulation); same operand / output conventions.
 // *nonfinite = 1 (and nothing written) when an operand holds Inf/NaN: the caller must use the exact kernel instead.
 cudaError_t tf32x3_gemm(const OzakiOperand* a_blocks, int na, const OzakiOperand* b_blocks, int nb, int64_t M, int64_t K, int64_t N,
@@ -535,8 +553,9 @@ struct SpgemmPair {
 struct SpgemmChain {
   int32_t m, n;           // frame dims of the output
   int32_t pair_begin, levels;
-  int32_t count_off;      // counters of level l: counts[count_off + l] = nnz(P_l), counts[count_off + levels + l] = nnz(S_l) - nnz(S_l-1)
-  int32_t pad;
+  int32_t count_off;      // counters of level l: counts[count_off + l] = nnz(P_l), counts[count_off + levels + l] = nnz(S_l) - nnz(S_l-1);
+                          // tri: then the same two counts over the diagonal at count_off + 2 levels and count_off + 3 levels
+  int32_t tri;            // a diagonal block of a Gram product: rows r <= c of column c only (its P_l are symmetric)
   int32_t* colcnt;        // count pass: [n] entries of each column of the final S
   const int32_t* optr;    // fill pass, sparse output: column pointers [n + 1] ...
   int32_t* oidx;          // ... row indices (nullptr: dense output) ...
@@ -549,18 +568,20 @@ struct SpgemmItem {       // one CTA's work: columns col0 .. col0 + spgemm_colum
 };
 struct SpgemmLaunchShape {
   int smem_counters;      // per-level counters in shared memory (levels <= this), else global atomics
+  int cnt_lines;          // counters per level: 2, or 4 when a chain is triangular
   bool acc_in_smem;       // per-warp column accumulators in shared memory, else in the caller's scratch (scratch_bytes)
   int max_ctas;           // persistent grid
   size_t scratch_bytes;
 };
 constexpr int kSpgemmMaxSmem = 200 * 1024;
 int spgemm_columns_per_item();
-SpgemmLaunchShape spgemm_shape(int max_m, int max_levels);
-// fill = false: the count pass (colcnt, counts, *d_products += scalar products; counts and products pre-zeroed);
-// fill = true: writes the entries.  Every chain's m <= max_m.
+SpgemmLaunchShape spgemm_shape(int max_m, int max_levels, bool tri);
+// fill = false: the count pass (colcnt, counts, *d_products += scalar products; counts and products pre-zeroed; *d_unsorted = 1
+// when d_unsorted is given and a walked R column's row indices do not ascend); fill = true: writes the entries.  Every chain's
+// m <= max_m.
 cudaError_t launch_spgemm(bool fill, const SpgemmItem* d_items, int nitems, const SpgemmChain* d_chains, const SpgemmPair* d_pairs,
                           int* d_counts, unsigned long long* d_products, void* d_scratch, int max_m, const SpgemmLaunchShape& s,
-                          cudaStream_t stream);
+                          int* d_unsorted, cudaStream_t stream);
 // out[0] = 0, out[t + 1] = in[0] + ... + in[t], t < n; one CTA per descriptor
 struct ScanDesc {
   const int32_t* in;

@@ -10,6 +10,11 @@
 // of the final sum, per-level nnz(P) and nnz(S) transitions, scalar products) and FILL (the entries, at column pointers scanned
 // from the counts, or a dense window).
 //
+// A triangular chain (SpgemmChain::tri: a diagonal block of a Gram product, whose every P_l is symmetric) accumulates only rows
+// r <= c of output column c, and its count pass also counts, per level, the diagonal entries of P_l and the zero <-> nonzero
+// transitions of S on the diagonal, so the host has the full block's counts (2 upper - diagonal).  Given an `unsorted` flag, the
+// count pass raises it when a walked R column's row indices do not ascend (DESIGN section 4.1.2: when a mirrored result is exact).
+//
 // sptrans_*: stable CSR <-> CSC conversion (the compressed arrays of a block's transpose), indices ascending in every line.
 #include <cub/block/block_scan.cuh>
 
@@ -47,35 +52,38 @@ __device__ __forceinline__ ColAcc acc_at(char* base, int M) {
   return a;
 }
 
+// cnt_lines: per-level counter lines of the launch (2, or 4 when a chain is triangular); smem_counters: levels per line in shared
+// memory (0: global atomics).  unsorted: nullptr, or the flag the count pass raises (see the file comment).
 template <bool FILL>
 __global__ void __launch_bounds__(kSpgemmWarps * 32, 1) spgemm_chain_kernel(const SpgemmItem* __restrict__ items, int nitems,
                                                                           const SpgemmChain* __restrict__ chains,
                                                                           const SpgemmPair* __restrict__ pairs, int* __restrict__ counts,
                                                                           unsigned long long* __restrict__ products, char* scratch,
-                                                                          int M, int smem_counters) {
+                                                                          int M, int smem_counters, int cnt_lines, int* unsorted) {
   extern __shared__ __align__(16) char spgemm_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const size_t acc_bytes = static_cast<size_t>(M) * (2 * sizeof(double) + 2 * sizeof(int));
-  int* cnt_smem = reinterpret_cast<int*>(spgemm_smem);  // [2 * smem_counters] when smem_counters > 0
+  int* cnt_smem = reinterpret_cast<int*>(spgemm_smem);  // [cnt_lines * smem_counters] when smem_counters > 0
   char* acc_base = scratch ? scratch + (static_cast<size_t>(blockIdx.x) * kSpgemmWarps + warp) * acc_bytes
-                           : spgemm_smem + static_cast<size_t>(2 * smem_counters) * sizeof(int) + warp * acc_bytes;
+                           : spgemm_smem + static_cast<size_t>(cnt_lines * smem_counters) * sizeof(int) + warp * acc_bytes;
   const ColAcc acc = acc_at(acc_base, M);
   for (int r = lane; r < M; r += 32) {
     acc.accS[r] = 0.0;
     acc.mark[r] = -1;
   }
   if (!FILL)
-    for (int t = threadIdx.x; t < 2 * smem_counters; t += blockDim.x) cnt_smem[t] = 0;
+    for (int t = threadIdx.x; t < cnt_lines * smem_counters; t += blockDim.x) cnt_smem[t] = 0;
   __syncthreads();
   int stamp = 0;
-  unsigned long long prod_count = 0;
+  unsigned long long prod_count = 0;  // per lane
   for (int it = blockIdx.x; it < nitems; it += gridDim.x) {
     const SpgemmItem item = items[it];
     const SpgemmChain& ch = chains[item.chain];
     const int L = ch.levels;
+    const bool tri = ch.tri != 0;
     const bool cnt_in_smem = !FILL && L <= smem_counters;
-    int* cntP = cnt_in_smem ? cnt_smem : counts + ch.count_off;
-    int* cntS = cntP + (cnt_in_smem ? smem_counters : L);
+    const int cstride = cnt_in_smem ? smem_counters : L;
+    int* cntP = cnt_in_smem ? cnt_smem : counts + ch.count_off;  // then nnz(S) steps, [tri] diagonal nnz(P), diagonal S steps
     for (int jj = warp; jj < kSpgemmCols; jj += kSpgemmWarps) {
       const int j = item.col0 + jj;
       if (j >= ch.n) break;
@@ -95,33 +103,43 @@ __global__ void __launch_bounds__(kSpgemmWarps * 32, 1) spgemm_chain_kernel(cons
         const double* __restrict__ rv = pairs[ch.pair_begin + l].rv;
         ++stamp;
         int nlist = 0;
+        int k_last = 0;  // the row index of the previous chunk's last entry
         for (int qc = q0; qc < q1; qc += 32) {
           // one stored R entry per lane: its row k, value b, and the range of L(:, k)
-          int a0 = 0, a1 = 0;
+          int a0 = 0, a1 = 0, k = 0;
           double b = 0.0;
           if (qc + lane < q1) {
-            const int k = ri[qc + lane];
+            k = ri[qc + lane];
             b = rv[qc + lane];
             a0 = lp[k];
             a1 = lp[k + 1];
+          }
+          if (!FILL && unsorted) {
+            const int up = __shfl_up_sync(0xffffffffu, k, 1);
+            const int prev = lane ? up : k_last;
+            if (qc + lane < q1 && (lane || qc > q0) && prev >= k) *unsorted = 1;
+            k_last = __shfl_sync(0xffffffffu, k, 31);
           }
           const int nq = min(32, q1 - qc);
           for (int t = 0; t < nq; ++t) {  // stored order of R(:, j)
             const int s0 = __shfl_sync(0xffffffffu, a0, t), s1 = __shfl_sync(0xffffffffu, a1, t);
             const double bb = __shfl_sync(0xffffffffu, b, t);
-            if (!FILL && lane == 0) prod_count += static_cast<unsigned long long>(s1 - s0);
             for (int e0 = s0; e0 < s1; e0 += 32) {
               const int e = e0 + lane;
-              bool first = false;
+              bool first = false, take = false;
               int i = 0;
               double p = 0.0;
               if (e < s1) {
                 i = li[e];
+                take = !tri || i <= j;  // a triangular chain: rows on and above the diagonal only
+              }
+              if (take) {
                 p = __dmul_rn(lv[e], bb);
                 first = acc.mark[i] != stamp;
               }
+              if (!FILL) prod_count += take;
               const unsigned fb = __ballot_sync(0xffffffffu, first);
-              if (e < s1) {
+              if (take) {
                 if (first) {
                   acc.mark[i] = stamp;
                   acc.list[nlist + __popc(fb & lanemask_lt())] = i;
@@ -136,7 +154,7 @@ __global__ void __launch_bounds__(kSpgemmWarps * 32, 1) spgemm_chain_kernel(cons
           }
         }
         // S(:, j) += P_l(:, j): each touched row once; count nnz(P_l) and the zero <-> nonzero transitions of S
-        int pc = 0, sd = 0;
+        int pc = 0, sd = 0, pdg = 0, sdg = 0;
         for (int t = lane; t < nlist; t += 32) {
           const int i = acc.list[t];
           const double p = acc.accP[i];
@@ -144,7 +162,12 @@ __global__ void __launch_bounds__(kSpgemmWarps * 32, 1) spgemm_chain_kernel(cons
             ++pc;
             const double s = acc.accS[i];
             const double ns = __dadd_rn(s, p);
-            sd += static_cast<int>(ns != 0.0) - static_cast<int>(s != 0.0);
+            const int step = static_cast<int>(ns != 0.0) - static_cast<int>(s != 0.0);
+            sd += step;
+            if (i == j) {  // read only for triangular chains
+              pdg = 1;
+              sdg = step;
+            }
             acc.accS[i] = ns;
           }
         }
@@ -155,27 +178,38 @@ __global__ void __launch_bounds__(kSpgemmWarps * 32, 1) spgemm_chain_kernel(cons
             pc += __shfl_xor_sync(0xffffffffu, pc, o);
             sd += __shfl_xor_sync(0xffffffffu, sd, o);
           }
+          if (tri) {
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+              pdg += __shfl_xor_sync(0xffffffffu, pdg, o);
+              sdg += __shfl_xor_sync(0xffffffffu, sdg, o);
+            }
+          }
           if (lane == 0) {
             if (pc) atomicAdd(cntP + l, pc);
-            if (sd) atomicAdd(cntS + l, sd);
+            if (sd) atomicAdd(cntP + cstride + l, sd);
+            if (tri && pdg) atomicAdd(cntP + 2 * cstride + l, pdg);
+            if (tri && sdg) atomicAdd(cntP + 3 * cstride + l, sdg);
           }
         }
       }
-      // the final column: rows ascending, entries != 0.0; accS is cleared for the next column
+      // the final column: rows ascending, entries != 0.0; accS is cleared for the next column.  A triangular chain ends at the
+      // diagonal (nothing below it was accumulated, and a dense window's lower part is the mirror pass's).
       int out = 0;
       const int base = FILL && ch.oidx ? ch.optr[j] : 0;
-      for (int r0 = 0; r0 < ch.m; r0 += 32) {
+      const int rows = tri ? min(ch.m, j + 1) : ch.m;
+      for (int r0 = 0; r0 < rows; r0 += 32) {
         const int r = r0 + lane;
         double v = 0.0;
-        if (r < ch.m) {
+        if (r < rows) {
           v = acc.accS[r];
           acc.accS[r] = 0.0;
         }
-        const bool nz = r < ch.m && v != 0.0;
+        const bool nz = r < rows && v != 0.0;
         const unsigned nb = __ballot_sync(0xffffffffu, nz);
         if (FILL) {
           if (ch.dense) {
-            if (r < ch.m) ch.dense[static_cast<int64_t>(r) * ch.drs + static_cast<int64_t>(j) * ch.dcs] = nz ? v : 0.0;
+            if (r < rows) ch.dense[static_cast<int64_t>(r) * ch.drs + static_cast<int64_t>(j) * ch.dcs] = nz ? v : 0.0;
           } else if (nz) {
             const int pos = base + out + __popc(nb & lanemask_lt());
             ch.oidx[pos] = r;
@@ -189,16 +223,20 @@ __global__ void __launch_bounds__(kSpgemmWarps * 32, 1) spgemm_chain_kernel(cons
     }
     if (cnt_in_smem) {  // flush this item's per-level counters
       __syncthreads();
-      for (int t = threadIdx.x; t < L; t += blockDim.x) {
-        if (cnt_smem[t]) atomicAdd(counts + ch.count_off + t, cnt_smem[t]);
-        if (cnt_smem[smem_counters + t]) atomicAdd(counts + ch.count_off + L + t, cnt_smem[smem_counters + t]);
-        cnt_smem[t] = 0;
-        cnt_smem[smem_counters + t] = 0;
-      }
+      const int lines = tri ? 4 : 2;
+      for (int t = threadIdx.x; t < L; t += blockDim.x)
+        for (int q = 0; q < lines; ++q) {
+          if (cnt_smem[q * smem_counters + t]) atomicAdd(counts + ch.count_off + q * L + t, cnt_smem[q * smem_counters + t]);
+          cnt_smem[q * smem_counters + t] = 0;
+        }
       __syncthreads();
     }
   }
-  if (!FILL && lane == 0 && prod_count) atomicAdd(products, prod_count);
+  if (!FILL) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) prod_count += __shfl_xor_sync(0xffffffffu, prod_count, o);
+    if (lane == 0 && prod_count) atomicAdd(products, prod_count);
+  }
 }
 
 // out[0] = 0, out[t + 1] = in[0] + ... + in[t]; one CTA per descriptor
@@ -268,8 +306,8 @@ __global__ void __launch_bounds__(256) sptrans_sort_kernel(const SpTransDesc* __
 PerDeviceOnce g_spgemm_attr;
 int g_sm_count[64] = {};
 
-size_t spgemm_smem_bytes(int M, int smem_counters, bool acc_in_smem) {
-  return static_cast<size_t>(2 * smem_counters) * sizeof(int) +
+size_t spgemm_smem_bytes(int M, int smem_counters, int cnt_lines, bool acc_in_smem) {
+  return static_cast<size_t>(cnt_lines * smem_counters) * sizeof(int) +
          (acc_in_smem ? static_cast<size_t>(kSpgemmWarps) * M * (2 * sizeof(double) + 2 * sizeof(int)) : 0);
 }
 
@@ -277,10 +315,11 @@ size_t spgemm_smem_bytes(int M, int smem_counters, bool acc_in_smem) {
 
 int spgemm_columns_per_item() { return kSpgemmCols; }
 
-SpgemmLaunchShape spgemm_shape(int max_m, int max_levels) {
+SpgemmLaunchShape spgemm_shape(int max_m, int max_levels, bool tri) {
   SpgemmLaunchShape s{};
   s.smem_counters = max_levels <= kSpgemmSmemCounters ? max_levels : 0;
-  s.acc_in_smem = spgemm_smem_bytes(max_m, s.smem_counters, true) <= kSpgemmMaxSmem;
+  s.cnt_lines = tri ? 4 : 2;
+  s.acc_in_smem = spgemm_smem_bytes(max_m, s.smem_counters, s.cnt_lines, true) <= kSpgemmMaxSmem;
   int dev = 0;
   cudaGetDevice(&dev);
   int sms = 132;
@@ -295,7 +334,7 @@ SpgemmLaunchShape spgemm_shape(int max_m, int max_levels) {
 
 cudaError_t launch_spgemm(bool fill, const SpgemmItem* d_items, int nitems, const SpgemmChain* d_chains, const SpgemmPair* d_pairs,
                           int* d_counts, unsigned long long* d_products, void* d_scratch, int max_m, const SpgemmLaunchShape& s,
-                          cudaStream_t stream) {
+                          int* d_unsorted, cudaStream_t stream) {
   if (nitems <= 0 || max_m <= 0) return cudaSuccess;
   cudaError_t e = g_spgemm_attr.run([&] {
     cudaError_t r = cudaFuncSetAttribute(spgemm_chain_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSpgemmMaxSmem);
@@ -304,14 +343,14 @@ cudaError_t launch_spgemm(bool fill, const SpgemmItem* d_items, int nitems, cons
   });
   if (e != cudaSuccess) return e;
   const int ctas = nitems < s.max_ctas ? nitems : s.max_ctas;
-  const size_t smem = spgemm_smem_bytes(max_m, fill ? 0 : s.smem_counters, s.acc_in_smem);
+  const size_t smem = spgemm_smem_bytes(max_m, fill ? 0 : s.smem_counters, s.cnt_lines, s.acc_in_smem);
   char* scratch = s.acc_in_smem ? nullptr : static_cast<char*>(d_scratch);
   if (fill)
     spgemm_chain_kernel<true><<<ctas, kSpgemmWarps * 32, smem, stream>>>(d_items, nitems, d_chains, d_pairs, d_counts, d_products, scratch,
-                                                                        max_m, 0);
+                                                                        max_m, 0, s.cnt_lines, nullptr);
   else
     spgemm_chain_kernel<false><<<ctas, kSpgemmWarps * 32, smem, stream>>>(d_items, nitems, d_chains, d_pairs, d_counts, d_products,
-                                                                         scratch, max_m, s.smem_counters);
+                                                                         scratch, max_m, s.smem_counters, s.cnt_lines, d_unsorted);
   return cudaGetLastError();
 }
 

@@ -36,3 +36,5 @@ run racecheck dspmm  "density_around_tau" tests/test_gpu_dspmm.py               
 run memcheck gram    "bit_for_bit and (640 or 700) or outliers_on_both_lines or absent_blocks" tests/test_gpu_gram.py  # shared residues, triangular tiles, upper-only fix-up, mirror
 run initcheck gram   "bit_for_bit and (640 or 700) or outliers_on_both_lines" tests/test_gpu_gram.py    # nothing reads a lower element no engine stored
 run racecheck gram   "bit_for_bit and 640" tests/test_gpu_gram.py                                        # the mirror kernel's shared tile
+run memcheck spgram  "layouts_and_densities and (0.004 or 0.06) and mixed or blk40 or absent_and_empty or single_block_8192 and 0.0004 or shuffled and csr" tests/test_gpu_sparse_gram.py  # triangular chains, sym completion, mirrors, fallback
+run racecheck spgram "layouts_and_densities and 0.02 and mixed" tests/test_gpu_sparse_gram.py            # per-level counters in shared memory
