@@ -88,7 +88,10 @@ MR_API mr_status mr_set_stream(mr_context* ctx, void* cuda_stream);
  *       "stream_budget_mb" (device memory a streamed multiply may use, in MiB; 0 = free device memory at the call minus 1 GiB),
  *       "oz2_ksplit" (the CTA-pair wgmma GEMM walks (modulus, K half, tile pair) work items -- half the L2 footprint of the
  *       residue panels in flight, bit-identical results: 1 = for long tile lists and K >= 8192 only, 2 = whenever possible; default 0,
- *       or the environment variable MATREL_OZ2_KSPLIT at mr_init) */
+ *       or the environment variable MATREL_OZ2_KSPLIT at mr_init),
+ *       "oz2_strassen" (1, the default: a resident Ozaki-II multiply of an even, full block grid with M, N, K >= 16384 runs one
+ *       level of Strassen per modulus -- seven half-size int8 residue products instead of eight, bit-identical results; 2 = at every
+ *       eligible size; 0 = off) */
 MR_API mr_status mr_set_option(mr_context* ctx, const char* key, int64_t value);
 MR_API mr_status mr_sync(mr_context* ctx);
 /* Orders the context stream (device side, no host wait) after every host->device block copy submitted so far. */
@@ -418,6 +421,8 @@ typedef struct mr_stats {
                                x sparse chains, those and the non-square blocks below it; 0 otherwise */
   int64_t gram_mirrored_blocks; /* blocks below the diagonal of that product written from their transposes (dense: the mirror pass;
                                sparse: square blocks, mirrored, sharing their transposes' arrays or converted from them) */
+  int64_t tc_strassen_jobs; /* Ozaki-II jobs of the most recent mr_matrix_multiply that ran one Strassen level (seven half-size
+                               residue products per modulus instead of eight; option "oz2_strassen") */
 } mr_stats;
 MR_API mr_status mr_get_stats(mr_context* ctx, mr_stats* out);
 MR_API mr_status mr_reset_stats(mr_context* ctx);

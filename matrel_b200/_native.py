@@ -87,6 +87,7 @@ class mr_stats(C.Structure):
         ("mv_sparse_entries", C.c_int64),
         ("gram_blocks", C.c_int64),           # blocks a Gram product computed (dense engines or sparse chains)
         ("gram_mirrored_blocks", C.c_int64),  # blocks below its diagonal written from their transposes
+        ("tc_strassen_jobs", C.c_int64),      # Ozaki-II jobs that ran one Strassen level (option oz2_strassen)
     ]
 
 

@@ -439,6 +439,7 @@ mr_status mr_set_option(mr_context* ctx, const char* key, int64_t value) {
     else if (k == "time_kernels") ctx->time_kernels = static_cast<int>(value);
     else if (k == "gemm_variant") ctx->force_variant = static_cast<int>(value);
     else if (k == "oz2_ksplit") ctx->oz2_ksplit = static_cast<int>(value);
+    else if (k == "oz2_strassen") ctx->oz2_strassen = static_cast<int>(value);
     else if (k == "pipeline") ctx->pipeline = static_cast<int>(value);
     else if (k == "stream_budget_mb") {
       MR_REQUIRE(value >= 0, MR_EINVAL, "stream_budget_mb must be >= 0, got %lld", (long long)value);

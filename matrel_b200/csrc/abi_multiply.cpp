@@ -348,6 +348,7 @@ struct Oz2Run {
   Buf d_maps;
   int cap_r = 0, cap_c = 0;
   int64_t int8_ops = 0;
+  bool strassen = false;  // the single job runs one Strassen level (DESIGN section 4.1.3)
 
   Oz2Run() = default;
   Oz2Run(const Oz2Run&) = delete;
@@ -358,9 +359,10 @@ struct Oz2Run {
   const int* flag() const { return eng ? oz2_flag(eng) : nullptr; }
 
   // Returns false when the multiply must stay on the exact kernel.  `group_of` may be rewritten to a single group (operands too
-  // large to keep every residue resident cannot be pipelined chunk by chunk).
+  // large to keep every residue resident cannot be pipelined chunk by chunk).  pipelined: operands are still arriving.
   bool plan(mr_context* c, const std::vector<OutPlan>& plans, const std::vector<size_t>& out_plan, const std::vector<double*>& cptr,
-            std::vector<int>& group_of, int& ngroups, int32_t blk, int64_t M, int64_t K, int64_t N, bool outer, bool guard, bool gram) {
+            std::vector<int>& group_of, int& ngroups, int32_t blk, int64_t M, int64_t K, int64_t N, bool outer, bool guard, bool gram,
+            bool pipelined) {
     ctx = c;
     if (M <= 0 || K <= 0 || N <= 0 || K >= (1 << 17) || out_plan.empty()) return false;
     const int T = oz2_moduli_for(K, ctx->crt_moduli);
@@ -482,8 +484,90 @@ struct Oz2Run {
                                     g.b->numCols, static_cast<uint8_t>(g.a->isT), static_cast<uint8_t>(g.b->isT), {0}});
       j.fouts.push_back(fo);
     };
+    // ---- one Strassen level (DESIGN section 4.1.3): a resident single-group product of an even grid of whole blocks, whose
+    // quadrants are whole 256-row tile pairs and 128-byte k-chunks, within the scratch budget at 7/4 of the plain residues.
+    // oz2_strassen = 1 takes it from M, N, K >= 16384 on (measured faster there; 4096^3 measured slower: the extra residue and CRT
+    // traffic outweighs an eighth of a short GEMM), 2 whenever it is eligible.
     int max_tiles = 1;
-    if (resident) {
+    const int nkb = static_cast<int>(K / blk);
+    constexpr int64_t kStrassenMinDim = 16384;
+    const bool big = M >= kStrassenMinDim && N >= kStrassenMinDim && K >= kStrassenMinDim;
+    strassen = (ctx->oz2_strassen >= 2 || (ctx->oz2_strassen == 1 && big)) && !outer && !gram && !share && resident && !pipelined && ngroups == 1 && blk % kOz2TileM == 0 &&
+               K % blk == 0 && nr % 2 == 0 && nc % 2 == 0 && nkb % 2 == 0 && M == static_cast<int64_t>(nr) * blk &&
+               N == static_cast<int64_t>(nc) * blk && (M / 2) % (2 * kOz2TileM) == 0 && (N / 2) % kOz2TileN == 0 && (K / 2) % 128 == 0 &&
+               out_plan.size() == static_cast<size_t>(nr) * nc;
+    std::vector<int2> pos;  // positions: tiles of a quadrant of C, in the banded order of finish_tiles
+    int pp = 0;             // positions per piece
+    if (strassen) {
+      std::set<std::pair<int, int>> ablk, bblk;  // (row, k) of A / (k, column) of B with a whole block
+      for (size_t oi : out_plan) {
+        const OutPlan& o = plans[oi];
+        if (o.m != blk || o.n != blk || o.pairs.size() != static_cast<size_t>(nkb)) strassen = false;
+        for (const PlanPair& g : o.pairs)
+          if (g.a->numRows == blk && g.a->numCols == blk && g.b->numCols == blk) {
+            ablk.insert({crow[o.rid], g.k});
+            bblk.insert({g.k, ccol[o.cid]});
+          }
+      }
+      strassen = strassen && ablk.size() == static_cast<size_t>(nr) * nkb && bblk.size() == static_cast<size_t>(nkb) * nc;
+    }
+    if (strassen) {
+      const int qtm = static_cast<int>(M / 2 / kOz2TileM), qtn = static_cast<int>(N / 2 / kOz2TileN);
+      for (int a = 0; a < qtm; ++a)
+        for (int b = 0; b < qtn; ++b) pos.push_back(make_int2(a, b));
+      std::sort(pos.begin(), pos.end(), [](const int2& x, const int2& y) {  // bands of 8 n-tiles, (2a, b) followed by (2a + 1, b)
+        if (x.y / 8 != y.y / 8) return x.y / 8 < y.y / 8;
+        if ((x.x >> 1) != (y.x >> 1)) return x.x < y.x;
+        if (x.y != y.y) return x.y < y.y;
+        return x.x < y.x;
+      });
+      // pieces of equal size: each holds the 7 sub-product tiles of its positions within the 2 GiB residue planes
+      const int npos = static_cast<int>(pos.size());
+      const int ppmax = static_cast<int>(std::min<int64_t>(npos, plane_cap_tiles / 7)) & ~1;
+      const int npieces = (npos + ppmax - 1) / ppmax;
+      pp = (npos + npieces - 1) / npieces;
+      pp += pp & 1;
+      size_t need = oz2_scratch_bytes(blk, K, T, nr, nc, 7 * pp, false, true);
+      const size_t budget = static_cast<size_t>(ctx->ozaki_scratch_mb > 0 ? ctx->ozaki_scratch_mb : 16384) << 20;
+      strassen = need <= budget;
+    }
+    if (strassen) {
+      Job j;
+      j.group = 0;
+      j.ctab.assign(static_cast<size_t>(cap_r) * cap_c, nullptr);
+      for (size_t t = 0; t < out_plan.size(); ++t) {
+        const OutPlan& o = plans[out_plan[t]];
+        const int cr = crow[o.rid], cc = ccol[o.cid];
+        j.ctab[static_cast<size_t>(cr) * cap_c + cc] = cptr[out_plan[t]];
+        add_fix(j, o, cptr[out_plan[t]], cr, cc);
+      }
+      // every slot at once, the blocks in quads of (line half, k half): (0, 0), (0, 1), (1, 0), (1, 1)
+      for (bool is_a : {true, false}) {
+        const int nl = is_a ? nr : nc;
+        std::vector<int> ids(nl);
+        for (int i = 0; i < nl; ++i) ids[i] = i;
+        Prep p = make_prep(is_a, ids, 0);
+        std::vector<const OzakiOperand*> at(static_cast<size_t>(nl) * nkb, nullptr);
+        for (const OzakiOperand& b : p.blocks) {
+          const int lb = (is_a ? b.row0 : b.col0) / blk, kb = (is_a ? b.col0 : b.row0) / blk;
+          at[static_cast<size_t>(lb) * nkb + kb] = &b;
+        }
+        std::vector<OzakiOperand> quads;
+        for (int lb = 0; lb < nl / 2; ++lb)
+          for (int kb = 0; kb < nkb / 2; ++kb)
+            for (int q = 0; q < 4; ++q) quads.push_back(*at[static_cast<size_t>(lb + (q >> 1) * (nl / 2)) * nkb + kb + (q & 1) * (nkb / 2)]);
+        p.blocks = std::move(quads);
+        j.preps.push_back(std::move(p));
+      }
+      // piece by piece, the 7 sub-products product-major
+      const int qtm = static_cast<int>(M / 2 / kOz2TileM), qtn = static_cast<int>(N / 2 / kOz2TileN);
+      for (size_t p0 = 0; p0 < pos.size(); p0 += pp)
+        for (int i = 0; i < 7; ++i)
+          for (size_t u = p0; u < std::min(pos.size(), p0 + pp); ++u) j.tiles.push_back(make_int2(i * qtm + pos[u].x, i * qtn + pos[u].y));
+      int8_ops += static_cast<int64_t>(j.tiles.size()) * T * 2ll * kOz2TileM * kOz2TileN * (Kpad / 2);
+      max_tiles = 7 * pp;
+      jobs.push_back(std::move(j));
+    } else if (resident) {
       std::vector<char> rprep(nr, 0), cprep(nc, 0);
       for (int gi = 0; gi < ngroups; ++gi) {
         Job j;
@@ -560,9 +644,11 @@ struct Oz2Run {
       }
     }
     if (jobs.empty()) return false;
-    max_tiles = static_cast<int>(std::min<int64_t>(max_tiles, plane_cap_tiles));
-    max_tiles += max_tiles & 1;
-    cudaError_t e = oz2_create(&eng, blk, K, T, cap_r, cap_c, max_tiles, guard ? 1 : 0, share, ctx->stream);
+    if (!strassen) {
+      max_tiles = static_cast<int>(std::min<int64_t>(max_tiles, plane_cap_tiles));
+      max_tiles += max_tiles & 1;
+    }
+    cudaError_t e = oz2_create(&eng, blk, K, T, cap_r, cap_c, max_tiles, guard ? 1 : 0, share, strassen, ctx->stream);
     if (e != cudaSuccess) {
       (void)cudaGetLastError();
       eng = nullptr;
@@ -1561,7 +1647,7 @@ void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const
   // The int8 tensor-core path (Ozaki-II residues + CRT) runs group by group in front of the DMMA launches, which then only execute
   // when the engine's device flag reports operands it cannot represent.  Small products stay on the exact kernel in auto mode.
   Oz2Run oz2;
-  const bool use_oz2 = dec.oz2 && oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0, gram);
+  const bool use_oz2 = dec.oz2 && oz2.plan(ctx, plans, out_plan, cptr, group_of, ngroups_dyn, blkSize, M, K, N, outer, algo == 0, gram, chunked);
   auto grp = [&](const Keyed& k) { return group_of[k.t.out]; };
   std::sort(keyed.begin(), keyed.end(), [&](const Keyed& x, const Keyed& y) {
     const int gx = grp(x), gy = grp(y);
@@ -1600,6 +1686,7 @@ void run_dense_engines(mr_context* ctx, const std::vector<OutPlan>& plans, const
     oz2.upload_tables();
     ctx->stats.tc_int8_ops = oz2.int8_ops;
     ctx->stats.tc_moduli = oz2_moduli(oz2.eng);
+    ctx->stats.tc_strassen_jobs = oz2.strassen ? static_cast<int64_t>(oz2.jobs.size()) : 0;
     ctx->stats.tc_gemm_launches += 1;
   }
   KernelTimer timer(ctx);
@@ -1981,6 +2068,7 @@ mr_status mr_matrix_multiply(mr_matrix* left, int64_t leftRowNum, int64_t leftCo
     ctx->stats.mv_sparse_entries = 0;
     ctx->stats.gram_blocks = 0;
     ctx->stats.gram_mirrored_blocks = 0;
+    ctx->stats.tc_strassen_jobs = 0;
     if (left->host || right->host)  // C tile by C tile through the device, into a host-resident result (abi_stream.cpp)
       *out = multiply_streamed(ctx, left, leftRowNum, leftColNum, right, rightRowNum, rightColNum, blkSize);
     else

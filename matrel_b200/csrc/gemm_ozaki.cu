@@ -868,6 +868,107 @@ __global__ void __launch_bounds__(256) residue_kernel(const OzBlock* __restrict_
   }
 }
 
+// ---- Ozaki-II with one level of Strassen (DESIGN section 4.1.3) ----------------------------------------------------------------
+// Quadrant (h, g) of an operand side: h = half of the lines (rows of A' / columns of B'), g = half of k.  In these terms A11 = (0, 0),
+// A12 = (0, 1), A21 = (1, 0), A22 = (1, 1), and B11 = (0, 0), B21 = (0, 1), B12 = (1, 0), B22 = (1, 1).  Operand i of the seven
+// products M1..M7 is sum_q coef[i][q] * quadrant q (q = 2 h + g):
+//   M1 = (A11 + A22)(B11 + B22)  M2 = (A21 + A22) B11  M3 = A11 (B12 - B22)  M4 = A22 (B21 - B11)  M5 = (A11 + A12) B22
+//   M6 = (A21 - A11)(B11 + B12)  M7 = (A12 - A22)(B21 + B22)
+__device__ constexpr int kStrassenA[7][4] = {{1, 0, 0, 1}, {0, 0, 1, 1}, {1, 0, 0, 0}, {0, 0, 0, 1}, {1, 1, 0, 0}, {-1, 0, 1, 0}, {0, 1, 0, -1}};
+__device__ constexpr int kStrassenB[7][4] = {{1, 0, 0, 1}, {1, 0, 0, 0}, {0, 0, 1, -1}, {-1, 1, 0, 0}, {0, 0, 0, 1}, {1, 0, 1, 0}, {0, 1, 0, 1}};
+
+// out_t[(i * lines_h + line) * Kh + k] = symmetric residue mod p_t of the exact integer operand i at local (line, k) of the quadrants.
+// blocks: four descriptors per quad (quadrants (0,0), (0,1), (1,0), (1,1)), each a whole block of the same size, gridDim.y = quads;
+// one CTA = 32 lines x 32 k of the quad.  Every element is scaled with the exponent of its own line, and the range guard records an
+// outlier once, with its original (line, k), and takes it as zero in every operand that uses it, exactly as residue_kernel does.  The
+// sums of at most two scaled elements stay within 2^(alpha + 1) <= 2^62 in magnitude (the engine takes the route for alpha <= 61
+// only), and the fold of residue_kernel holds for any magnitude below 2^64.
+template <bool IS_A>
+__global__ void __launch_bounds__(256, 2) strassen_residue_kernel(const OzBlock* __restrict__ blocks, const int32_t* __restrict__ line_exp,
+                                                               int8_t* __restrict__ out, size_t slice_stride, int Kh, int lines_h, int T,
+                                                               int alpha, int tiles_k_max, int* __restrict__ gate, int range_bits,
+                                                               OutlierRec* __restrict__ recs, int* __restrict__ rec_cnt, int sstride) {
+  __shared__ double sm[4][32][33];
+  if (gate != nullptr && *gate != 0) return;
+  const int tl = blockIdx.x / tiles_k_max, tk = blockIdx.x % tiles_k_max;
+  const int l0 = tl * 32, k0 = tk * 32;
+  const OzBlock* quad = blocks + 4 * static_cast<size_t>(blockIdx.y);
+  const int nlines = IS_A ? quad[0].rows : quad[0].cols, nks = IS_A ? quad[0].cols : quad[0].rows;
+  if (l0 >= nlines || k0 >= nks) return;
+  const int tid = threadIdx.x;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const OzBlock& b = quad[q];
+    const bool k_fast = IS_A ? (b.isT != 0) : (b.isT == 0);
+    for (int idx = tid; idx < 32 * 32; idx += 256) {
+      const int l = k_fast ? idx / 32 : idx % 32, k = k_fast ? idx % 32 : idx / 32;
+      sm[q][l][k] = IS_A ? blk_at(b, l0 + l, k0 + k) : blk_at(b, k0 + k, l0 + l);
+    }
+  }
+  __syncthreads();
+  const int l = tid >> 3, kq = (tid & 7) * 4;
+  long long X[4][4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const OzBlock& b = quad[q];
+    const int gl = (IS_A ? b.row0 : b.col0) + l0 + l, gk = (IS_A ? b.col0 : b.row0) + k0 + kq;
+    const int e = line_exp[gl];
+    const int sh1 = min(alpha - e, 1023);
+    const double line_scale = scalbn(1.0, sh1), line_scale2 = scalbn(1.0, alpha - e - sh1);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      double xv = sm[q][l][kq + j];
+      if (range_bits > 0 && xv != 0.0 && exponent_of(xv) < e - 1 - range_bits) {
+        const int slot = gl / sstride;
+        const int at = atomicAdd(&rec_cnt[slot], 1);
+        if (at < OZ2_REC_CAP) recs[static_cast<size_t>(slot) * OZ2_REC_CAP + at] = OutlierRec{gl, gk + j, xv};
+        else *gate = 1;
+        xv = 0.0;
+      }
+      X[q][j] = __double2ll_rn(xv * line_scale * line_scale2);
+    }
+  }
+  const CrtConst& cc = c_crt[T];
+  const int line = (IS_A ? quad[0].row0 : quad[0].col0) + l0 + l, k = (IS_A ? quad[0].col0 : quad[0].row0) + k0 + kq;
+  const float kMagic = 12582912.0f;
+#pragma unroll
+  for (int i = 0; i < 7; ++i) {
+    uint32_t hi[4], lo[4];
+    float sgn[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      long long Y = 0;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int c = IS_A ? kStrassenA[i][q] : kStrassenB[i][q];
+        if (c > 0) Y += X[q][j];
+        else if (c < 0) Y -= X[q][j];
+      }
+      sgn[j] = Y < 0 ? -1.0f : 1.0f;
+      const unsigned long long U = Y < 0 ? 0ull - static_cast<unsigned long long>(Y) : static_cast<unsigned long long>(Y);
+      hi[j] = static_cast<uint32_t>(U >> 32);
+      lo[j] = static_cast<uint32_t>(U);
+    }
+    int8_t* dst0 = out + (static_cast<size_t>(i) * lines_h + line) * Kh + k;
+    for (int t = 0; t < T; ++t) {  // the fold of residue_kernel
+      const float pf = static_cast<float>(cc.p[t]);
+      const uint32_t wl = cc.clo[t], wh = cc.chi[t];
+      const float ip = cc.invpf[t];
+      uint32_t bytes[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t x = __dp4a(lo[j], wl, __dp4a(hi[j], wh, 0u));
+        const float f = __uint_as_float(0x4B000000u | x) - 8388608.0f;
+        const float q = __fadd_rn(__fmaf_rn(f, ip, kMagic), -kMagic);
+        const float r = __fmaf_rn(-q, pf, f);
+        bytes[j] = __float_as_uint(__fmaf_rn(r, sgn[j], kMagic));
+      }
+      *reinterpret_cast<uint32_t*>(dst0 + static_cast<size_t>(t) * slice_stride) =
+          __byte_perm(__byte_perm(bytes[0], bytes[1], 0x0040), __byte_perm(bytes[2], bytes[3], 0x0040), 0x5410);
+    }
+  }
+}
+
 // CRT reconstruction: one CTA = 32 rows x 128 columns of one 128 x 256 tile of the job (8 CTAs per tile).  Thread (row, 4 columns)
 // reads its T residue quads (coalesced along the compact plane rows) and accumulates S = sum_t r_t w_t in fp64, EXACTLY: every
 // weight is split into 40-bit chunks (c_crtf), so each chunk sum stays an integer below 2^52 (r < 2^8, T <= 2^4).  With
@@ -889,22 +990,56 @@ __device__ __forceinline__ double scale_by_pow2(double x, int n) {
   return x;
 }
 
-template <int NCH>
+//
+// STR (the Strassen route): the piece's tile list holds the 7 sub-products product-major, npos positions each, so its first npos
+// entries are the positions (local tiles of a quadrant of C).  CTA = (position, quadrant of C, 32 x 128 part); the quadrant's 2 or 4
+// sub-product residues are combined modulo p into [0, p) before the same exact sum, so every output bit is that of the plain route:
+//   C11 = M1 + M4 - M5 + M7   C12 = M3 + M5   C21 = M2 + M4   C22 = M1 - M2 + M3 + M6
+// The 4 quadrants of a position are neighbouring CTAs, so a sub-product tile that several of them read comes from L2 after the first.
+struct StrCrt {
+  int npos;        // positions of the piece
+  int qtm, qtn;    // tiles per quadrant of C: 128-row tiles, 256-column tiles
+};
+// sub-products (M1..M7 as 0..6) of the quadrants of C, as the terms a, b, c, d of str_byte
+__constant__ int c_str_terms[4][4] = {{0, 3, 4, 6}, {2, 4, 0, 0}, {1, 3, 0, 0}, {0, 2, 1, 5}};
+// (a + b + d - c) mod p per byte for four residue bytes in [0, p) each (c = 0: (a + b) mod p)
+__device__ __forceinline__ uint32_t str_byte(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t pm, bool four, int j) {
+  const uint32_t sel = 0x4440u + j;
+  uint32_t s = __byte_perm(a, 0u, sel) + __byte_perm(b, 0u, sel);
+  if (four) {
+    s += __byte_perm(d, 0u, sel) + pm - __byte_perm(c, 0u, sel);  // < 4 p
+    s = min(s, s - 2 * pm);
+  }
+  return min(s, s - pm);
+}
+
+template <int NCH, bool STR>
 __global__ void __launch_bounds__(256) crt_kernel(const int8_t* __restrict__ planes, size_t plane_stride, int T,
                                                   const int2* __restrict__ tiles, const int32_t* __restrict__ row_exp,
                                                   const int32_t* __restrict__ col_exp, int two_alpha, double* const* __restrict__ ctab,
                                                   const int32_t* __restrict__ rdims, const int32_t* __restrict__ cdims, int sstride,
-                                                  int ncslots, const int* __restrict__ gate) {
+                                                  int ncslots, const int* __restrict__ gate, StrCrt sc) {
   __shared__ double tile[128][33];
   if (gate != nullptr && *gate != 0) return;
   const CrtF& cf = c_crtf[T];
-  const int t_idx = blockIdx.x >> 3, sub = blockIdx.x & 7;
-  const int2 tl = tiles[t_idx];
+  const int t_idx = STR ? blockIdx.x >> 5 : blockIdx.x >> 3, sub = blockIdx.x & 7;
+  int2 tl = tiles[t_idx];
+  const int quadrant = (blockIdx.x >> 3) & 3;
+  if (STR) {
+    tl.x += (quadrant >> 1) * sc.qtm;
+    tl.y += (quadrant & 1) * sc.qtn;
+  }
   const int r0t = (sub >> 1) * 32, c0t = (sub & 1) * 128;  // inside the tile
   const int r0 = tl.x * BM + r0t, c0 = tl.y * BN + c0t;     // buffer coordinates
   const int tid = threadIdx.x;
   const int lr = tid >> 5, lc = (tid & 31) * 4;  // 8 rows per pass, 4 passes
   const int8_t* tbase = planes + static_cast<size_t>(t_idx) * (BM * BN);
+  // STR: the plane tiles of the quadrant's sub-products, as offsets from tbase: a + b + d - c (four) or a + b
+  const bool four = quadrant == 0 || quadrant == 3;
+  size_t toff[4] = {0, 0, 0, 0};
+  if (STR)
+#pragma unroll
+    for (int u = 0; u < 4; ++u) toff[u] = static_cast<size_t>(c_str_terms[quadrant][u]) * sc.npos * (BM * BN);
   constexpr double kTwo52 = 4503599627370496.0, kMagic = 6755399441055744.0;  // 2^52, 1.5 * 2^52
   constexpr double kUp = 1099511627776.0, kDown = 1.0 / 1099511627776.0;        // 2^40, 2^-40
 #pragma unroll 1
@@ -918,11 +1053,28 @@ __global__ void __launch_bounds__(256) crt_kernel(const int8_t* __restrict__ pla
     const int8_t* src = tbase + static_cast<size_t>(r0t + pass * 8 + lr) * BN + c0t + lc;
 #pragma unroll 4
     for (int t = 0; t < T; ++t) {
-      const uint32_t quad = *reinterpret_cast<const uint32_t*>(src + static_cast<size_t>(t) * plane_stride);
+      const int8_t* st = src + static_cast<size_t>(t) * plane_stride;
+      uint32_t res[4];
+      if (STR) {
+        const uint32_t a = *reinterpret_cast<const uint32_t*>(st + toff[0]), b = *reinterpret_cast<const uint32_t*>(st + toff[1]);
+        const uint32_t pm = c_crt[T].p[t];
+        if (four) {
+          const uint32_t c = *reinterpret_cast<const uint32_t*>(st + toff[2]), d = *reinterpret_cast<const uint32_t*>(st + toff[3]);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) res[j] = str_byte(a, b, c, d, pm, true, j);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) res[j] = str_byte(a, b, 0u, 0u, pm, false, j);
+        }
+      } else {
+        const uint32_t quad = *reinterpret_cast<const uint32_t*>(st);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) res[j] = __byte_perm(quad, 0u, 0x4440u + j);
+      }
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         // byte j as a double: 2^52 + r has r in its low mantissa bits
-        const double x = __hiloint2double(0x43300000, static_cast<int>(__byte_perm(quad, 0u, 0x4440u + j))) - kTwo52;
+        const double x = __hiloint2double(0x43300000, static_cast<int>(res[j])) - kTwo52;
 #pragma unroll
         for (int i = 0; i < NCH; ++i) S[j][i] = fma(x, cf.w[t][i], S[j][i]);
       }
@@ -1467,6 +1619,8 @@ struct Oz2Engine {
                    // long tile lists and deep K only, 2 = whenever K has an even number of chunks (tests)
   bool paired = false;   // tile lists hold vertically adjacent 128-row tiles in pairs: the CTA-pair kernel runs them
   bool share_ab = false; // Gram product: A' is the first Mpad lines of B', and the A side reads the B side's tables (a_line0)
+  bool strassen = false; // one Strassen level: A' is [7 Mpad / 2][Kpad / 2] per modulus (sub-product i in lines [i Mpad / 2, ...)),
+                         // B' likewise; tile lists hold the 7 sub-products of each piece product-major (DESIGN section 4.1.3)
   int64_t K = 0, Kpad = 0, Mpad = 0, Npad = 0;
   size_t a_stride = 0, b_stride = 0, plane_stride = 0;
   int8_t *As = nullptr, *Bs = nullptr, *planes = nullptr;
@@ -1507,11 +1661,12 @@ int oz2_moduli_for(int64_t K, int requested) {
   return CRT_MAX_T;
 }
 
-size_t oz2_scratch_bytes(int blk, int64_t K, int T, int cap_r, int cap_c, int max_tiles, bool share_ab) {
+size_t oz2_scratch_bytes(int blk, int64_t K, int T, int cap_r, int cap_c, int max_tiles, bool share_ab, bool strassen) {
   const int64_t sstride = (blk + BM - 1) / BM * BM;
   const int64_t Kpad = (K + BKB - 1) / BKB * BKB;
   const int64_t Mpad = share_ab ? 0 : sstride * cap_r, Npad = (sstride * cap_c + BN - 1) / BN * BN;
-  return static_cast<size_t>(T) * (Mpad + Npad) * Kpad + static_cast<size_t>(T) * max_tiles * (BM * BN);
+  const size_t res = static_cast<size_t>(T) * (Mpad + Npad) * Kpad;
+  return (strassen ? res / 4 * 7 : res) + static_cast<size_t>(T) * max_tiles * (BM * BN);
 }
 
 int oz2_tiles_per_block(int blk) {
@@ -1521,13 +1676,17 @@ int oz2_tiles_per_block(int blk) {
 
 // Creates the engine and its scratch (stream-ordered allocations).  cap_r / cap_c = row / column slots held at once.
 cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, int guard_range,
-                       bool share_ab, cudaStream_t stream) {
+                       bool share_ab, bool strassen, cudaStream_t stream) {
   *out = nullptr;
   const int T = oz2_moduli_for(K, moduli);
   int log2P[CRT_MAX_T + 1];
   OZ_CHECK(crt_constants(log2P));
   int alpha = crt_alpha(log2P[T], K);
   if (alpha < 8 || K >= (1 << 17) || cap_r <= 0 || cap_c <= 0 || max_tiles <= 0 || (share_ab && cap_r != cap_c))
+    return cudaErrorInvalidValue;
+  // Strassen: whole 256-row tile pairs and 128-byte k-chunks per half, exact int64 sums of two scaled elements
+  if (strassen && (share_ab || blk % BM != 0 || (static_cast<int64_t>(blk) * cap_r) % (2 * BN) != 0 ||
+                   (static_cast<int64_t>(blk) * cap_c) % (2 * BN) != 0 || K % (2 * BKB) != 0 || alpha > 61 || max_tiles % 7 != 0))
     return cudaErrorInvalidValue;
   std::unique_ptr<Oz2Engine> e(new Oz2Engine);
   e->T = T;
@@ -1539,6 +1698,7 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
   e->cap_c = cap_c;
   e->max_tiles = max_tiles;
   e->share_ab = share_ab;
+  e->strassen = strassen;
   // auto mode: every non-zero element must keep >= 18 bits after the per-line scaling, which bounds the error of every product
   // term by 2^-17 of the term itself, i.e. the result by 2^-17 |A||B| element-wise (north-star tolerance 1e-5) in the worst
   // case; data of ordinary dynamic range sees the full alpha bits (1e-14 .. 1e-16)
@@ -1549,6 +1709,10 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
   e->Npad = (static_cast<int64_t>(e->sstride) * cap_c + BN - 1) / BN * BN;
   e->a_stride = static_cast<size_t>(e->Mpad) * e->Kpad;
   e->b_stride = static_cast<size_t>(e->Npad) * e->Kpad;
+  if (strassen) {
+    e->a_stride = e->a_stride / 4 * 7;
+    e->b_stride = e->b_stride / 4 * 7;
+  }
   e->plane_stride = static_cast<size_t>(max_tiles) * (BM * BN);
   OZ_CHECK(configure_gemm_kernels());
   int dev = 0;
@@ -1580,11 +1744,13 @@ cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_
   // tensor maps: A' (box 128 rows), B' (box 256 rows: single-CTA kernel), B' (box 128 rows: each CTA of a pair loads half).
   // Shared residues: row slot s of A' is column slot s of B' (Mpad <= Npad)
   e->h_maps.resize(static_cast<size_t>(3 * T) * 128);
+  const uint64_t mk = strassen ? e->Kpad / 2 : e->Kpad;
+  const uint64_t ma = strassen ? e->Mpad / 2 * 7 : e->Mpad, mb = strassen ? e->Npad / 2 * 7 : e->Npad;
   for (int t = 0; t < T; ++t) {
     int8_t* a_plane = share_ab ? e->Bs + e->b_stride * t : e->As + e->a_stride * t;
-    if (!make_i8_map(&e->h_maps[static_cast<size_t>(t) * 128], a_plane, e->Kpad, e->Mpad, BM) ||
-        !make_i8_map(&e->h_maps[static_cast<size_t>(T + t) * 128], e->Bs + e->b_stride * t, e->Kpad, e->Npad, BN) ||
-        !make_i8_map(&e->h_maps[static_cast<size_t>(2 * T + t) * 128], e->Bs + e->b_stride * t, e->Kpad, e->Npad, BN / 2)) {
+    if (!make_i8_map(&e->h_maps[static_cast<size_t>(t) * 128], a_plane, mk, ma, BM) ||
+        !make_i8_map(&e->h_maps[static_cast<size_t>(T + t) * 128], e->Bs + e->b_stride * t, mk, mb, BN) ||
+        !make_i8_map(&e->h_maps[static_cast<size_t>(2 * T + t) * 128], e->Bs + e->b_stride * t, mk, mb, BN / 2)) {
       Oz2Engine* raw = e.release();
       oz2_destroy(raw, stream);
       return cudaErrorInvalidValue;
@@ -1626,6 +1792,8 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
                         int nslots, const int32_t* d_dims, bool need_zero, cudaStream_t stream) {
   if (nslots <= 0) return cudaSuccess;
   if (slot0 < 0 || slot0 + nslots > (is_a ? e->cap_r : e->cap_c) || (is_a && e->share_ab)) return cudaErrorInvalidValue;
+  // Strassen: every slot at once, from whole blocks in quads (see strassen_residue_kernel)
+  if (e->strassen && (slot0 != 0 || nslots != (is_a ? e->cap_r : e->cap_c) || need_zero || nblocks % 4 != 0)) return cudaErrorInvalidValue;
   static_assert(sizeof(OzakiOperand) == sizeof(OzBlock), "OzakiOperand is the device block descriptor");
   const OzBlock* blocks = reinterpret_cast<const OzBlock*>(d_blocks);
   const size_t line0 = (is_a ? 0 : static_cast<size_t>(e->Mpad)) + static_cast<size_t>(slot0) * e->sstride;
@@ -1653,7 +1821,22 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
                                                                                e->bad);
   OZ_CHECK(cudaGetLastError());
   e->launches += 1;
-  if (nblocks > 0) {
+  if (nblocks > 0 && e->strassen) {
+    const int max_l = is_a ? max_rows : max_cols, max_k = is_a ? max_cols : max_rows;
+    const int tk = (max_k + 31) / 32, tl = (max_l + 31) / 32;
+    const int lines_h = static_cast<int>((is_a ? e->Mpad : e->Npad) / 2), Kh = static_cast<int>(e->Kpad / 2);
+    OutlierRec* recs = e->recs + static_cast<size_t>(is_a ? 0 : e->cap_r) * OZ2_REC_CAP;
+    int* rec_cnt = e->rec_cnt + (is_a ? 0 : e->cap_r);
+    OZ_CHECK(for_block_chunks(nblocks / 4, [&](int off, int cnt) {
+      if (is_a)
+        strassen_residue_kernel<true><<<dim3(tl * tk, cnt), 256, 0, stream>>>(blocks + 4 * off, exps, res, stride, Kh, lines_h, e->T, e->alpha,
+                                                                              tk, e->bad, e->range_bits, recs, rec_cnt, e->sstride);
+      else
+        strassen_residue_kernel<false><<<dim3(tl * tk, cnt), 256, 0, stream>>>(blocks + 4 * off, exps, res, stride, Kh, lines_h, e->T, e->alpha,
+                                                                               tk, e->bad, e->range_bits, recs, rec_cnt, e->sstride);
+    }));
+    e->launches += 1;
+  } else if (nblocks > 0) {
     // "line" = row of A / column of B, "k" = the other index
     const int max_l = is_a ? max_rows : max_cols, max_k = is_a ? max_cols : max_rows;
     const int tk = (max_k + 127) / 128, tl = (max_l + 31) / 32;
@@ -1674,6 +1857,7 @@ cudaError_t oz2_prepare(Oz2Engine* e, bool is_a, const OzakiOperand* d_blocks, i
 // residue GEMM launch time (events, synchronises): used for the roofline figure only.
 void oz2_set_ksplit(Oz2Engine* e, int level) { e->ksplit = level; }
 void oz2_set_paired(Oz2Engine* e, bool paired) { e->paired = paired && (e->max_tiles % 2 == 0) && (e->Mpad % (2 * BM) == 0); }
+bool oz2_strassen(const Oz2Engine* e) { return e->strassen; }
 bool oz2_paired(const Oz2Engine* e) { return e->paired; }
 
 cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* const* d_ctab, cudaStream_t stream, double* ms_gemm,
@@ -1681,15 +1865,18 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
   if (ntiles <= 0) return cudaSuccess;
   if (e->d_maps == nullptr) return cudaErrorInvalidValue;
   if (e->paired && (ntiles & 1)) return cudaErrorInvalidValue;
+  // Strassen: each piece is 7 sub-products x npos positions (max_tiles = 7 x the positions of a whole piece), of half the K
+  if (e->strassen && ntiles % 7 != 0) return cudaErrorInvalidValue;
+  const int64_t kg = e->strassen ? e->Kpad / 2 : e->Kpad;
   OzakiGemmParams p{};
   p.tmaps = e->d_maps;
-  p.Kpad = static_cast<int32_t>(e->Kpad);
+  p.Kpad = static_cast<int32_t>(kg);
   p.kstep = BKB;
   p.kc0 = 0;
-  p.nkc = static_cast<int32_t>(e->Kpad / BKB);
+  p.nkc = static_cast<int32_t>(kg / BKB);
   p.npairs = 1;
-  p.tiles_m = static_cast<int32_t>(e->Mpad / BM);
-  p.tiles_n = static_cast<int32_t>(e->Npad / BN);
+  p.tiles_m = static_cast<int32_t>((e->strassen ? e->Mpad / 2 * 7 : e->Mpad) / BM);
+  p.tiles_n = static_cast<int32_t>((e->strassen ? e->Npad / 2 * 7 : e->Npad) / BN);
   p.nmod = e->T;
   p.planes = e->planes;
   p.plane_stride = e->plane_stride;
@@ -1724,10 +1911,13 @@ cudaError_t oz2_multiply(Oz2Engine* e, const int2* d_tiles, int ntiles, double* 
       OZ_CHECK(cudaEventElapsedTime(&ms, ev0, ev1));
       *ms_gemm += ms;
     }
-    auto crt = e->crt_chunks == 3 ? crt_kernel<3> : crt_kernel<4>;
-    crt<<<static_cast<unsigned>(cnt) * 8u, 256, 0, stream>>>(e->planes, e->plane_stride, e->T, d_tiles + off, e->exps + e->a_line0(),
-                                                              e->exps + e->Mpad, 2 * e->alpha, d_ctab, e->dims + e->a_slot0(),
-                                                              e->dims + e->cap_r, e->sstride, e->cap_c, e->bad);
+    StrCrt sc{cnt / 7, static_cast<int>(e->Mpad / 2 / BM), static_cast<int>(e->Npad / 2 / BN)};
+    auto crt = e->strassen ? (e->crt_chunks == 3 ? crt_kernel<3, true> : crt_kernel<4, true>)
+                           : (e->crt_chunks == 3 ? crt_kernel<3, false> : crt_kernel<4, false>);
+    // Strassen: 4 output tiles (the quadrants of C) per position
+    const unsigned ctas = e->strassen ? static_cast<unsigned>(sc.npos) * 32u : static_cast<unsigned>(cnt) * 8u;
+    crt<<<ctas, 256, 0, stream>>>(e->planes, e->plane_stride, e->T, d_tiles + off, e->exps + e->a_line0(), e->exps + e->Mpad, 2 * e->alpha,
+                                  d_ctab, e->dims + e->a_slot0(), e->dims + e->cap_r, e->sstride, e->cap_c, e->bad, sc);
     OZ_CHECK(cudaGetLastError());
     e->launches += 2;
   }

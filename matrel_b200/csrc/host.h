@@ -92,6 +92,8 @@ struct mr_context {
   int spmm_algo = 0;         // 0 = auto (pipelined TMA kernel when the blocks are large enough), 1 = the simple shared-memory kernel
   int time_kernels = 0;
   int force_variant = -1;
+  int oz2_strassen = 1;   // option "oz2_strassen": one Strassen level for eligible resident Ozaki-II multiplies (DESIGN section 4.1.3):
+                          // 1 = from M, N, K >= 16384 on, 2 = at every eligible size, 0 = off
   int oz2_ksplit = 0;     // option "oz2_ksplit" (default: environment MATREL_OZ2_KSPLIT, else 0): K-split item order of the CTA-pair GEMM
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev_alloc = nullptr, ev_order = nullptr;
   cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;  // ingest / egress overlap with compute on `stream`

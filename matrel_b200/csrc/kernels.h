@@ -91,11 +91,16 @@ cudaError_t ozaki_gemm_f64(const OzakiOperand* a_blocks, int na, const OzakiOper
 // engine's remaining kernels are no-ops then and the caller's gated DMMA launch produces the blocks instead.
 struct Oz2Engine;
 // share_ab: a Gram product (left = right^T, cap_r == cap_c): the A side of slot s is the B side of slot s, so only the B' residues
-// are held (one operand's scratch) and preparing a B slot also makes its A slot
-size_t oz2_scratch_bytes(int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, bool share_ab = false);
+// are held (one operand's scratch) and preparing a B slot also makes its A slot.
+// strassen: one Strassen level (DESIGN section 4.1.3).  Every slot is prepared at once, from whole blocks given in quads (quadrants
+// (0,0), (0,1), (1,0), (1,1) of (line half, k half)); a tile list is cut into pieces of max_tiles = 7 x positions, each holding the
+// 7 sub-products product-major: sub-product i of position (lm, ln) (a tile of a quadrant of C) is the buffer tile
+// (i Mpad / 256 + lm, i Npad / 512 + ln).  The residue scratch is 7/4 of the plain one.
+size_t oz2_scratch_bytes(int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, bool share_ab = false, bool strassen = false);
 int oz2_tiles_per_block(int blk);
 cudaError_t oz2_create(Oz2Engine** out, int blk, int64_t K, int moduli, int cap_r, int cap_c, int max_tiles, int guard_range,
-                       bool share_ab, cudaStream_t stream);
+                       bool share_ab, bool strassen, cudaStream_t stream);
+bool oz2_strassen(const Oz2Engine* e);
 void oz2_destroy(Oz2Engine* e, cudaStream_t stream);
 const void* oz2_host_maps(const Oz2Engine* e, size_t* bytes);   // 2 * moduli CUtensorMaps to be uploaded by the caller ...
 void oz2_set_device_maps(Oz2Engine* e, const void* d_maps);     // ... and handed back as a device pointer
